@@ -68,8 +68,9 @@ typedef struct {
     /* image state (ImageState :176-186) */
     real *final_T, *hit_normal_c, *hit_point_c, *weight_sum;
     int32_t *n_contrib;
-    /* copies of the inputs the backward re-reads */
-    const real *means, *shs, *opac, *scales, *rots;
+    /* copies of the inputs the backward re-reads; colors_precomp replaces shs and cov3D_precomp replaces
+     * scales / rots when given (NULL otherwise) */
+    const real *means, *shs, *opac, *scales, *rots, *colors_precomp, *cov3D_precomp;
 } OracleState;
 
 /* ------------------------------------------------------------------ helpers */
@@ -229,9 +230,17 @@ int oracle_sizeof_real(void) { return (int)sizeof(real); }
  * Rasterizer::forward, rasterizer_impl.cu:205-437, with the output
  * initialisation of RasterizeGaussiansCUDA (rasterize_points.cu:79-87).
  * `tie` (H*W bytes, may be NULL) is set where a discrete per-pixel decision
- * was within v->tie_eps (relative) of flipping.                              */
+ * was within v->tie_eps (relative) of flipping.
+ * colors_precomp (P*3, or NULL) replaces the SH colour (forward.cu:330,
+ * rasterizer_impl.cu:365): not clamped, clamp flags stay 0. cov3D_precomp
+ * (P*6, or NULL) replaces computeCov3D (forward.cu:289-291); scales and rots
+ * are then not read. The reference defines no depth side in that mode (its
+ * render kernel reads scales[] unconditionally, forward.cu:779, while its
+ * Python API forbids passing scales with cov3D_precomp): a hit Gaussian gets
+ * no surfel, so its depth is the centre depth.                               */
 OracleState *oracle_forward(const OracleView *v, int P, int M, const real *means, const real *shs, const real *opac,
-                            const real *scales, const real *rots, const int32_t *tile_mask, real *out_color,
+                            const real *scales, const real *rots, const real *colors_precomp, const real *cov3D_precomp,
+                            const int32_t *tile_mask, real *out_color,
                             real *out_depth, int32_t *out_hit_color, int32_t *out_hit_depth, real *out_hit_color_w,
                             real *out_hit_depth_w, real *out_T, int32_t *radii_out, uint8_t *tie, int nthreads) {
     const int H = v->H, W = v->W, N = H * W;
@@ -239,6 +248,7 @@ OracleState *oracle_forward(const OracleView *v, int P, int M, const real *means
     OracleState *s = (OracleState *)calloc(1, sizeof(OracleState));
     s->P = P; s->M = M; s->H = H; s->W = W; s->tiles_x = gx; s->tiles_y = gy; s->v = *v;
     s->means = means; s->shs = shs; s->opac = opac; s->scales = scales; s->rots = rots;
+    s->colors_precomp = colors_precomp; s->cov3D_precomp = cov3D_precomp;
     s->depth = (real *)calloc((size_t)P + 1, sizeof(real));
     s->xy = (real *)calloc((size_t)2 * P + 2, sizeof(real));
     s->conic_o = (real *)calloc((size_t)4 * P + 4, sizeof(real));
@@ -282,7 +292,8 @@ OracleState *oracle_forward(const OracleView *v, int P, int M, const real *means
         xform4x3(p, v->view, pv);
         if (pv[2] <= (real)0.2f || pp[0] < -1.3 || pp[0] > 1.3 || pp[1] < -1.3 || pp[1] > 1.3) continue;
         real *c6 = s->cov3D + 6 * idx;
-        cov3d_from(scales + 3 * idx, v->scale_modifier, rots + 4 * idx, c6);
+        if (cov3D_precomp) memcpy(c6, cov3D_precomp + 6 * idx, 6 * sizeof(real));
+        else cov3d_from(scales + 3 * idx, v->scale_modifier, rots + 4 * idx, c6);
         real A[2][3], t[3], V[3][3];
         ewa_A(p, v->view, focal_x, focal_y, v->tanfovx, v->tanfovy, A, t, NULL, NULL);
         sym6_to_mat(c6, V);
@@ -309,7 +320,8 @@ OracleState *oracle_forward(const OracleView *v, int P, int M, const real *means
         int x0, y0, x1, y1;
         get_rect(pix[0], pix[1], (int)my_radius, gx, gy, &x0, &y0, &x1, &y1);
         if ((x1 - x0) * (y1 - y0) == 0) continue;
-        sh_to_rgb(v->sh_degree, M, p, v->campos, shs + (size_t)3 * M * idx, s->rgb + 3 * idx, s->clamped + 3 * idx);
+        if (colors_precomp) memcpy(s->rgb + 3 * idx, colors_precomp + 3 * idx, 3 * sizeof(real));
+        else sh_to_rgb(v->sh_degree, M, p, v->campos, shs + (size_t)3 * M * idx, s->rgb + 3 * idx, s->clamped + 3 * idx);
         s->depth[idx] = pv[2];
         s->radii[idx] = (int)my_radius;
         s->xy[2 * idx] = pix[0]; s->xy[2 * idx + 1] = pix[1];
@@ -415,7 +427,12 @@ OracleState *oracle_forward(const OracleView *v, int P, int M, const real *means
                     if (eps > 0 && near_rel(alpha, (real)(1.0f / 255.0f), eps)) flag = 1;
                     if (alpha < (real)(1.0f / 255.0f)) continue;
                     if (!hit && eps > 0 && near_rel(alpha, v->opaque_threshold, eps)) flag = 1;
-                    if (!hit && alpha >= v->opaque_threshold) {
+                    if (!hit && alpha >= v->opaque_threshold && cov3D_precomp) {
+                        hit_id = g; /* no surfel: centre depth */
+                        hit_dw = alpha * Tcur;
+                        depth_ = s->depth[g];
+                        hit = 1;
+                    } else if (!hit && alpha >= v->opaque_threshold) {
                         /* forward.cu:778-809; computeNormal_ScaleMax :54-74 */
                         real Rm[3][3];
                         const real *sc = scales + 3 * g;
@@ -612,8 +629,12 @@ void oracle_backward(const OracleState *s, const real *dL_dpix, const real *dL_d
                     a_con[4 * g + 3] += (real)-0.5f * gdy * dy * dL_dG;
                     a_op[g] += G * dL_dalpha;
                 }
-                /* depth-hit gradient, backward.cu:997-1065 */
-                if (hit_image[pix_id] >= 0) {
+                /* depth-hit gradient, backward.cu:997-1065; without a surfel (cov3D_precomp) the centre depth's */
+                if (hit_image[pix_id] >= 0 && s->cov3D_precomp) {
+                    int g = hit_image[pix_id];
+                    real dLd = dL_ddepth[pix_id];
+                    add3(a_m3 + 3 * g, dLd * v->view[2], dLd * v->view[6], dLd * v->view[10]);
+                } else if (hit_image[pix_id] >= 0) {
                     int g = hit_image[pix_id];
                     real ray[3];
                     pixel_ray(px, py, focal_x, focal_y, v->cx, v->cy, ray);
@@ -732,8 +753,8 @@ void oracle_backward(const OracleState *s, const real *dL_dpix, const real *dL_d
              (pj[4] * mw - pj[7] * mul1) * g2x + (pj[5] * mw - pj[7] * mul2) * g2y,
              (pj[8] * mw - pj[11] * mul1) * g2x + (pj[9] * mw - pj[11] * mul2) * g2y);
 
-        /* computeColorFromSH bwd, backward.cu:152-268 */
-        {
+        /* computeColorFromSH bwd, backward.cu:152-268; skipped for precomputed colours (:539) */
+        if (!s->colors_precomp) {
             const real *sh = s->shs + (size_t)3 * M * idx;
             real *dsh = dL_dsh + (size_t)3 * M * idx;
             real dir0[3] = {mean[0] - v->campos[0], mean[1] - v->campos[1], mean[2] - v->campos[2]};
@@ -789,8 +810,8 @@ void oracle_backward(const OracleState *s, const real *dL_dpix, const real *dL_d
             add3(dL_dmeans3D + 3 * idx, dmx, dmy, dmz);
         }
 
-        /* computeCov3D bwd, backward.cu:426-487 */
-        {
+        /* computeCov3D bwd, backward.cu:426-487; skipped for a precomputed covariance (:546) */
+        if (!s->cov3D_precomp) {
             const real *q = s->rots + 4 * idx, *sc = s->scales + 3 * idx;
             real Rm[3][3];
             quat_to_R(q, Rm);

@@ -59,13 +59,17 @@ DEFAULTS = dict(  # SLAM/render.py:33-49,83-87 + configs/base.yaml:65-68
 
 
 def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
 class OracleRender:
-    """One forward evaluation; keeps the state `backward` needs (like the reference's ctx)."""
+    """One forward evaluation; keeps the state `backward` needs (like the reference's ctx).
 
-    def __init__(self, cam, g, tile_mask=None, precision="f32", tie_eps=0.0, nthreads=0, **settings):
+    `colors_precomp` (P,3) replaces the SH colour of g["shs"], `cov3D_precomp` (P,6) the covariance of g["scales"] /
+    g["rotations"] (GaussianRasterizer's alternative inputs); the replaced entries of `g` are then not read."""
+
+    def __init__(self, cam, g, tile_mask=None, precision="f32", tie_eps=0.0, nthreads=0, colors_precomp=None,
+                 cov3D_precomp=None, **settings):
         lib, real = _lib(precision)
         self.lib, self.real, self.precision = lib, real, precision
         dt = np.float32 if precision == "f32" else np.float64
@@ -92,12 +96,14 @@ class OracleRender:
         V.tie_eps = tie_eps
         self.V = V
         self.P = P = g["xyz"].shape[0]
-        self.M = M = g["shs"].shape[1]
+        arr = lambda a, *shape: None if a is None else np.ascontiguousarray(a, dtype=dt).reshape(P, *shape)
+        self.colors_precomp, self.cov3D_precomp = arr(colors_precomp, 3), arr(cov3D_precomp, 6)
         self.means = np.ascontiguousarray(g["xyz"], dtype=dt)
-        self.shs = np.ascontiguousarray(g["shs"], dtype=dt)
+        self.shs = arr(g["shs"], *g["shs"].shape[1:]) if colors_precomp is None else None
+        self.M = M = self.shs.shape[1] if self.shs is not None else 0
         self.opac = np.ascontiguousarray(g["opacity"], dtype=dt).reshape(-1)
-        self.scales = np.ascontiguousarray(g["scales"], dtype=dt)
-        self.rots = np.ascontiguousarray(g["rotations"], dtype=dt)
+        self.scales = arr(g["scales"], 3) if cov3D_precomp is None else None
+        self.rots = arr(g["rotations"], 4) if cov3D_precomp is None else None
         th, tw = (H + 15) // 16, (W + 15) // 16
         if tile_mask is None:
             tile_mask = np.ones((th, tw), dtype=np.int32)
@@ -114,7 +120,7 @@ class OracleRender:
         self.tie = np.zeros((H, W), np.uint8)
         self.state = lib.oracle_forward(
             C.byref(V), C.c_int(P), C.c_int(M), _p(self.means), _p(self.shs), _p(self.opac), _p(self.scales), _p(self.rots),
-            _p(self.tile_mask), _p(self.color), _p(self.depth), _p(self.hit_color), _p(self.hit_depth),
+            _p(self.colors_precomp), _p(self.cov3D_precomp), _p(self.tile_mask), _p(self.color), _p(self.depth), _p(self.hit_color), _p(self.hit_depth),
             _p(self.hit_color_weight), _p(self.hit_depth_weight), _p(self.T_map), _p(self.radii),
             _p(self.tie) if tie_eps > 0 else None, C.c_int(nthreads))
         self.num_rendered = int(lib.oracle_num_rendered(self.state))
@@ -145,7 +151,9 @@ class OracleRender:
         return fT.reshape(self.H, self.W), nc.reshape(self.H, self.W)
 
     def backward(self, dL_dcolor, dL_ddepth, nthreads=0):
-        """Returns dict of grads w.r.t. (means3D, shs, opacities, scales, rotations) + the 2-D intermediates."""
+        """Returns dict of grads w.r.t. (means3D, shs, opacities, scales, rotations) + the 2-D intermediates. With
+        precomputed colours "colors_precomp" (= the intermediate "colors") replaces "shs"; with a precomputed covariance
+        "cov3D_precomp" (= the intermediate "cov3D") replaces "scales" and "rotations"."""
         P, M, dt = self.P, self.M, self.dt
         gc = np.ascontiguousarray(dL_dcolor, dtype=dt)
         gd = np.ascontiguousarray(dL_ddepth, dtype=dt)
@@ -155,6 +163,12 @@ class OracleRender:
         self.lib.oracle_backward(C.c_void_p(self.state), _p(gc), _p(gd), _p(self.hit_depth), _p(out["means3D"]), _p(out["shs"]),
                                  _p(out["opacities"]), _p(out["scales"]), _p(out["rotations"]), _p(out["means2D"]),
                                  _p(out["conic"]), _p(out["colors"]), _p(out["cov3D"]), C.c_int(nthreads))
+        if self.colors_precomp is not None:
+            del out["shs"]
+            out["colors_precomp"] = out["colors"]
+        if self.cov3D_precomp is not None:
+            del out["scales"], out["rotations"]
+            out["cov3D_precomp"] = out["cov3D"]
         return out
 
     def close(self):

@@ -180,7 +180,10 @@ def _f32_cuda(t, name, device):
         raise TypeError(f"{name} must be a CUDA float32 tensor (got {t.dtype} on {t.device})")
     if t.device != device:
         raise ValueError(f"{name} is on {t.device}, expected {device}")
-    return t.contiguous()
+    t = t.contiguous()
+    # the kernels read rotations and 16-coefficient SH rows with 128-bit loads; a view at an offset into its storage may
+    # be contiguous and still misaligned
+    return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
 def _make_view(rs: GaussianRasterizationSettings, device) -> tuple[RtgSplatView, tuple]:
@@ -227,6 +230,8 @@ def _forward_native(rs, means3D, sh, colors_precomp, opacities, scales, rotation
     if tile_mask.numel() != th * tw:
         raise ValueError(f"tile_mask must have {th}x{tw} entries")
     M = sh.size(1) if sh is not None else 0
+    if sh is not None and (int(rs.sh_degree) + 1) ** 2 > M:
+        raise ValueError(f"sh_degree {int(rs.sh_degree)} needs {(int(rs.sh_degree) + 1) ** 2} SH coefficients per Gaussian, shs has {M}")
     view, keep = _make_view(rs, device)
     stream = torch.cuda.current_stream(device).cuda_stream  # fetched per call: autograd runs backward on its own thread
 
@@ -329,6 +334,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                 t = buf[name]
                 if t.numel() != int(torch.Size(shape).numel()) or t.dtype != torch.float32 or t.device != device or not t.is_contiguous():
                     raise ValueError(f"grad buffer '{name}' must be a contiguous float32 tensor of {tuple(shape)} on {device}")
+                if t.data_ptr() % 16:
+                    raise ValueError(f"grad buffer '{name}' must start at a 16-byte aligned address (the kernels store 128 bits at a time)")
                 return t.view(shape)
             return torch.empty(shape, **f32)
         g_means = out("means3D", (P, 3))

@@ -12,6 +12,7 @@ from rtg_slam_b200 import scene
 
 import helpers
 from golden.make_raster_golden import CASES, build_case
+from golden.make_raster_inputs_golden import CASES as INPUT_CASES, build_case as build_input_case
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 NAMES = ("color", "depth", "hit_color", "hit_depth", "hit_color_weight", "hit_depth_weight", "T_map", "radii")
@@ -129,3 +130,96 @@ def test_oracle_matches_reference_cuda_golden(name):
         jitter = float(gold["jitter_" + k])
         tol = max(1e-3, 10 * jitter)
         assert helpers.rel_err(gr[k], gold["grad_" + k]) < tol, (k, helpers.rel_err(gr[k], gold["grad_" + k]), jitter)
+
+
+COLOR_SIDE = ("color", "hit_color", "hit_color_weight", "T_map", "radii")
+
+
+def test_precomputed_colors_reproduce_the_sh_run(room):
+    """colors_precomp equal to the SH run's colours renders identically; dL/dcolors_precomp is that run's dL/dcolors."""
+    cam, g = room
+    g64 = {k: v.astype(np.float64) for k, v in g.items()}
+    gc, gd = scene.upstream_grads(cam)
+    base = OracleRender(cam, g64, precision="f64")
+    o = OracleRender(cam, g64, precision="f64", colors_precomp=base.geom()["rgb"])
+    for k, v in outputs(base).items():
+        assert np.array_equal(outputs(o)[k], v), k
+    gb, go = base.backward(gc, gd), o.backward(gc, gd)
+    assert "shs" not in go and np.abs(gb["colors"]).max() > 0
+    # the backward sums per-thread partial gradients in a varying order: equal to f64 rounding
+    assert helpers.rel_err(go["colors_precomp"], gb["colors"]) < 1e-12
+    for k in ("opacities", "scales", "rotations", "means2D", "conic"):
+        assert helpers.rel_err(go[k], gb[k]) < 1e-12, k
+
+
+def test_precomputed_covariance_reproduces_the_scale_rotation_run(room):
+    """cov3D_precomp equal to the run's own covariance: identical colour side and dL/dcov3D. Without scales there is no
+    surfel, so the depth of a hit is the centre depth."""
+    cam, g = room
+    g64 = {k: v.astype(np.float64) for k, v in g.items()}
+    gc, gd = scene.upstream_grads(cam)
+    base = OracleRender(cam, g64, precision="f64")
+    o = OracleRender(cam, g64, precision="f64", cov3D_precomp=base.geom()["cov3D"])
+    for k in COLOR_SIDE + ("hit_depth", "hit_depth_weight"):
+        assert np.array_equal(outputs(o)[k], outputs(base)[k]), k
+    hit = o.hit_depth[0] >= 0
+    assert hit.any()
+    assert np.array_equal(o.depth[0][hit], o.geom()["depth"][o.hit_depth[0][hit]])
+    gb, go = base.backward(gc, gd), o.backward(gc, gd)
+    assert "scales" not in go and "rotations" not in go and np.abs(gb["cov3D"]).max() > 0
+    assert helpers.rel_err(go["cov3D_precomp"], gb["cov3D"]) < 1e-12
+    for k in ("opacities", "shs", "means2D", "conic"):
+        assert helpers.rel_err(go[k], gb[k]) < 1e-12, k
+
+
+def test_precomputed_input_gradients_match_finite_differences(room):
+    cam, g = room
+    g64 = {k: v.astype(np.float64) for k, v in g.items()}
+    gc, gd = scene.upstream_grads(cam)
+    ref = OracleRender(cam, g64, precision="f64")
+    geom = ref.geom()
+    rng = np.random.default_rng(1)
+    vis = np.where(ref.radii > 0)[0]
+    # colours outside [0, 1] as well: precomputed colours are not clamped
+    cols = geom["rgb"] + rng.uniform(-0.3, 0.3, geom["rgb"].shape)
+    for key, val in (("colors_precomp", cols), ("cov3D_precomp", geom["cov3D"])):
+        base = OracleRender(cam, g64, precision="f64", **{key: val})
+        an = base.backward(gc, gd)
+        for name, x in (("xyz", None), (key, val)):
+            for _ in range(4):
+                i = int(rng.choice(vis))
+                arr = g64[name] if x is None else x
+                idx = (i,) + tuple(int(rng.integers(0, s)) for s in arr.shape[1:])
+                h = 1e-6 * max(1e-2, abs(arr[idx]))
+                vals = []
+                for sgn in (1, -1):
+                    a = arr.copy()
+                    a[idx] += sgn * h
+                    gm, kw = (dict(g64, xyz=a), {key: val}) if x is None else (g64, {key: a})
+                    o = OracleRender(cam, gm, precision="f64", **kw)
+                    vals.append(float((o.color * gc).sum() + (o.depth * gd).sum()))
+                    o.close()
+                fd = (vals[0] - vals[1]) / (2 * h)
+                a_ = an["means3D" if x is None else key][idx]
+                assert abs(fd - a_) <= 1e-4 * max(abs(fd), abs(a_)) + 1e-9, (key, name, idx, fd, a_)
+
+
+@pytest.mark.parametrize("name", sorted(INPUT_CASES))
+def test_oracle_matches_reference_cuda_golden_alternative_inputs(name):
+    """Precomputed colours and a 4-coefficient SH table against the reference's own CUDA rasterizer."""
+    path = os.path.join(GOLD, name + ".npz")
+    if not os.path.exists(path):
+        pytest.skip("golden fixture not generated yet (needs a GPU run of make_raster_inputs_golden.py)")
+    gold = np.load(path)
+    cam, inputs, mask, grads, over = build_input_case(name)
+    g = {k: inputs.get(k) for k in ("xyz", "opacity", "shs", "scales", "rotations")}
+    o = OracleRender(cam, g, tile_mask=mask, precision="f32", tie_eps=1e-4, colors_precomp=inputs.get("colors_precomp"), **over)
+    st = helpers.compare_outputs(outputs(o), {k: gold[k] for k in NAMES}, tie=o.tie, tol=1e-4, label=name)
+    assert st["radii_mismatch"] == 0
+    assert o.num_rendered == int(gold["num_rendered"])
+    gr = o.backward(*grads)
+    keys = [k[len("grad_"):] for k in gold.files if k.startswith("grad_")]
+    assert ("colors_precomp" in keys) == ("colors_precomp" in inputs) and len(keys) == 5
+    for k in keys:
+        tol = max(1e-3, 10 * float(gold["jitter_" + k]))
+        assert helpers.rel_err(gr[k], gold["grad_" + k]) < tol, (k, helpers.rel_err(gr[k], gold["grad_" + k]))

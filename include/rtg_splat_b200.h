@@ -113,6 +113,25 @@ int rtg_splat_backward_visible(const RtgSplatView *view, int32_t P, int32_t M, c
                                float *dL_dmeans3D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
                                float *dL_dscales, float *dL_drotations, float *dL_dcov3D, float *dL_dmeans2D, void *stream);
 
+/* rtg_splat_backward (visible_rows_only == 0) or rtg_splat_backward_visible (!= 0) that also differentiates the camera:
+ * the per-Gaussian gradients are those of the extended call, and `dL_dcamera` (device, 35 floats, all written) receives
+ * dL/dviewmatrix (16, the storage order of `view->viewmatrix`), dL/dprojmatrix (16) and dL/dcampos (3) -- the plain
+ * elementwise derivative of the same loss with respect to the arrays the forward read, for any matrices it accepts.
+ * Entries the forward never reads (viewmatrix 3, 7, 11, 15) get 0; intrinsics and the discrete decisions (culling,
+ * tile cut-off, alpha < 1/255, opaque hit, plane test) are not differentiated. `camera_scratch`: caller-owned device
+ * memory of rtg_splat_camera_scratch_bytes(P) bytes, 8-byte aligned, for the per-block partial sums; the reduction has a
+ * fixed order, so identical gradient records give a bit-identical dL_dcamera. Whole-map calls only (no tile-sharded
+ * exchange step). */
+size_t rtg_splat_camera_scratch_bytes(int32_t P);
+int rtg_splat_backward_camera(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                              const float *colors_precomp, const float *scales, const float *rotations,
+                              const float *cov3D_precomp, const int32_t *radii, const void *geom_ws, const void *img_ws,
+                              const void *bin_ws, int64_t R_cap, const int32_t *counters, const float *final_T,
+                              const int32_t *hit_image, const float *dL_dcolor, const float *dL_ddepth, float *grad2d_scratch,
+                              float *dL_dmeans3D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity,
+                              float *dL_dscales, float *dL_drotations, float *dL_dcov3D, float *dL_dmeans2D,
+                              int32_t visible_rows_only, float *dL_dcamera, void *camera_scratch, void *stream);
+
 /* The same backward in two calls with the same argument list, for callers that put an exchange step between the
  * compositing backward and the per-Gaussian backward (tile-sharded multi-GPU rendering, SURVEY.md section 8(e)):
  *   rtg_splat_backward_render : zero-fill of the culled rows + backward of renderCUDA (backward.cu:808-1066); on return

@@ -75,6 +75,8 @@ SIGNATURES = {
     "rtg_splat_backward_visible": (C.c_int, _BWD_ARGS),
     "rtg_splat_backward_render": (C.c_int, _BWD_ARGS),
     "rtg_splat_backward_finish": (C.c_int, _BWD_ARGS),
+    "rtg_splat_camera_scratch_bytes": (C.c_size_t, [_I32]),
+    "rtg_splat_backward_camera": (C.c_int, _BWD_ARGS[:-1] + [_I32, _VP, _VP, _VP]),
     "rtg_splat_geom_layout": (C.c_int, [_I32] + [C.POINTER(C.c_size_t)] * 4),
     "rtg_splat_forward_preprocess": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32, _I32, _I32] + [_VP] * 7 + [_VP, _VP, _I64, _VP, _VP]),
     "rtg_splat_forward_render": (C.c_int, [C.POINTER(RtgSplatView), _I32, _VP, _VP, _VP, _VP, _I64] + [_VP] * 7 + [_VP, _VP, _VP, _VP, _I32, _I32, _VP]),

@@ -331,11 +331,18 @@ static int splat_backward_impl(int phase, int32_t p_begin, int32_t p_end, const 
                        const int32_t *radii, const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap,
                        const int32_t *counters, const float *final_T, const int32_t *hit_image, const float *dL_dcolor, const float *dL_ddepth, float *grad2d_scratch,
                        float *dL_dmeans3D, float *dL_dsh, float *dL_dcolors_precomp, float *dL_dopacity, float *dL_dscales,
-                       float *dL_drotations, float *dL_dcov3D, float *dL_dmeans2D, void *stream) {
+                       float *dL_drotations, float *dL_dcov3D, float *dL_dmeans2D, void *stream, float *dL_dcamera = nullptr,
+                       void *camera_scratch = nullptr) {
     int rc = validate_view(view, "rtg_splat_backward");
     if (rc) return rc;
     if (P < 0 || p_begin < 0 || p_end < p_begin || p_end > P) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_splat_backward: bad P / range");
-    if (P == 0) return RTG_OK;
+    if (P == 0) {
+        if (!dL_dcamera) return RTG_OK;
+        // nothing visible: the camera gradient is zero
+        cudaError_t e = cudaMemsetAsync(dL_dcamera, 0, 35 * sizeof(float), reinterpret_cast<cudaStream_t>(stream));
+        if (e != cudaSuccess) return fail(RTG_ERR_CUDA, std::string("rtg_splat_backward_camera memset: ") + cudaGetErrorString(e));
+        return RTG_OK;
+    }
     if (!means3D || !radii || !geom_ws || !img_ws || !bin_ws || !counters || !final_T || !hit_image || !dL_dcolor || !dL_ddepth ||
         !grad2d_scratch || !dL_dmeans3D || !dL_dopacity)
         return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_splat_backward: NULL pointer");
@@ -375,7 +382,11 @@ static int splat_backward_impl(int phase, int32_t p_begin, int32_t p_end, const 
         rtg::launch_render_bwd(vp, g, b, img, counters, final_T, hit_image, dL_dcolor, dL_ddepth, grad2d_scratch, s);
         if (forked) cudaStreamWaitEvent(s, ss->join, 0);  // enqueued after both: the zero-fill still overlaps render_bwd
     }
-    if (phase != 1)  // walks the compact visible list, which holds only Gaussians of [p_begin, p_end)
+    if (dL_dcamera)  // whole map only (p_begin == 0): the per-Gaussian backward that also reduces the camera terms
+        rtg::launch_preprocess_bwd_camera(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count, grad2d_scratch,
+                                          dL_dmeans3D, dL_dsh, dL_dcolors_precomp, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D,
+                                          dL_dmeans2D, dL_dcamera, camera_scratch, s);
+    else if (phase != 1)  // walks the compact visible list, which holds only Gaussians of [p_begin, p_end)
         rtg::launch_preprocess_bwd(vp, p_end - p_begin, M, shift_rows(means3D, p_begin, 3), shift_rows(scales, p_begin, 3),
                                    shift_rows(rotations, p_begin, 4), shift_rows(shs, p_begin, (size_t)3 * M),
                                    shift_rows(cov3D_precomp, p_begin, 6), g, b.vis_count, grad2d_scratch,
@@ -401,6 +412,26 @@ int rtg_splat_backward(RTG_BWD_PARAMS) { return splat_backward_impl(0, 0, P, RTG
 int rtg_splat_backward_visible(RTG_BWD_PARAMS) { return splat_backward_impl(3, 0, P, RTG_BWD_ARGS); }
 int rtg_splat_backward_render(RTG_BWD_PARAMS) { return splat_backward_impl(1, 0, P, RTG_BWD_ARGS); }
 int rtg_splat_backward_finish(RTG_BWD_PARAMS) { return splat_backward_impl(2, 0, P, RTG_BWD_ARGS); }
+size_t rtg_splat_camera_scratch_bytes(int32_t P) { return P < 0 ? 0 : rtg::camera_scratch_bytes(P); }
+
+int rtg_splat_backward_camera(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                              const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                              const int32_t *radii, const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap,
+                              const int32_t *counters, const float *final_T, const int32_t *hit_image, const float *dL_dcolor,
+                              const float *dL_ddepth, float *grad2d_scratch, float *dL_dmeans3D, float *dL_dsh,
+                              float *dL_dcolors_precomp, float *dL_dopacity, float *dL_dscales, float *dL_drotations,
+                              float *dL_dcov3D, float *dL_dmeans2D, int32_t visible_rows_only, float *dL_dcamera,
+                              void *camera_scratch, void *stream) {
+    int rc = validate_view(view, "rtg_splat_backward_camera");
+    if (rc) return rc;
+    if (P < 0) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_splat_backward_camera: P < 0");
+    if (!dL_dcamera || !camera_scratch)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_splat_backward_camera: dL_dcamera / camera_scratch is NULL");
+    if (((uintptr_t)camera_scratch) & 7)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_splat_backward_camera: camera_scratch must be 8-byte aligned");
+    return splat_backward_impl(visible_rows_only ? 3 : 0, 0, P, RTG_BWD_ARGS, dL_dcamera, camera_scratch);
+}
+
 int rtg_splat_backward_render_shard(int32_t p_begin, int32_t p_end, RTG_BWD_PARAMS) {
     return splat_backward_impl(1, p_begin, p_end, RTG_BWD_ARGS);
 }

@@ -16,6 +16,14 @@ void launch_preprocess_bwd(const ViewParams &vp, int P, int M, const float *mean
                            const float *shs, const float *cov3D_precomp, const GeomState &g, const uint32_t *vis_count, float *rec,
                            float *dL_dmeans, float *dL_dsh, float *dL_dcolors, float *dL_dopacity, float *dL_dscales, float *dL_drot,
                            float *dL_dcov3D, float *dL_dmeans2D, cudaStream_t s);
+// launch_preprocess_bwd that also writes dL/d(viewmatrix 16, projmatrix 16, campos 3) to `dL_dcamera` (35 floats, device);
+// `camera_scratch`: camera_scratch_bytes(P) bytes of device memory for the block partials
+size_t camera_scratch_bytes(int P);
+void launch_preprocess_bwd_camera(const ViewParams &vp, int P, int M, const float *means, const float *scales, const float *rots,
+                                  const float *shs, const float *cov3D_precomp, const GeomState &g, const uint32_t *vis_count,
+                                  float *rec, float *dL_dmeans, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
+                                  float *dL_dscales, float *dL_drot, float *dL_dcov3D, float *dL_dmeans2D, float *dL_dcamera,
+                                  void *camera_scratch, cudaStream_t s);
 
 // binning.cu
 void launch_tile_histogram(const ViewParams &vp, int P, const GeomState &g, const int *radii, const int *tile_mask, const BinState &b,

@@ -443,11 +443,18 @@ __device__ __forceinline__ float3 bwd_sh(const int deg, const int idx, const int
     return dmean;
 }
 
+// Camera terms of one Gaussian (CAMERA variant of bwd_visible), RTG_CAM_TERMS floats:
+//   [3j+k]      j < 4, k < 3   dL/dviewmatrix[4j+k]          (view[4j+3] is never read: its gradient is 0)
+//   [12+3j+c]   j < 4, c < 3   dL/dprojmatrix[4j+{0,1,3}[c]] (proj[4j+2] only feeds the cull and the unused NDC z: 0)
+//   [24+i]      i < 3          dL/dcampos[i]
+#define RTG_CAM_TERMS 27
+
+template <bool CAMERA>
 __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx, const int M, const float *s_m,
                                             const float *__restrict__ means, const float *__restrict__ scales,
                                             const float *__restrict__ rots, const float *__restrict__ shs,
                                             const float *__restrict__ cov3D_precomp, const GeomState &g, float *__restrict__ rec,
-                                            const BwdOut &o) {
+                                            const BwdOut &o, float *cam) {
     const float *vm = s_m, *pj = s_m + 16;
     const size_t i3 = 3 * (size_t)idx;
     const bool has_sh = (shs != nullptr);
@@ -480,6 +487,9 @@ __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx,
         const float3 dsh_mean = bwd_sh(vp.sh_degree, idx, M, mean, make_float3(s_m[32], s_m[33], s_m[34]), dcol[0], dcol[1], dcol[2],
                                        __float_as_int(g.rgb_flags[idx].w), shs, dL_dsh);
         dmean.x += dsh_mean.x; dmean.y += dsh_mean.y; dmean.z += dsh_mean.z;
+        if constexpr (CAMERA) {  // campos enters only through the view direction mean - campos
+            cam[24] = -dsh_mean.x; cam[25] = -dsh_mean.y; cam[26] = -dsh_mean.z;
+        }
     }
     float3 sc = make_float3(0.f, 0.f, 0.f);
     float4 q = make_float4(1.f, 0.f, 0.f, 0.f);
@@ -600,6 +610,43 @@ __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx,
         reinterpret_cast<float4 *>(dL_drot)[idx] = drot;
     }
 
+    if constexpr (CAMERA) {
+        // The view matrix enters through the view-space centre p = W mean + T (the EWA J path `dt` and the depth path),
+        // through W in A = J W, and through the view-space surfel normal W n. The record holds the depth path's view-space
+        // gradients pulled back to world space (W^T dpc, W^T dnc, render.cu depth_hit_grad): W^-T (s_m[36..44], row
+        // major) recovers them, for any invertible W.
+        const float *wi = s_m + 36;
+        const float3 dpc = make_float3(wi[0] * rc.y + wi[1] * rc.z + wi[2] * rc.w, wi[3] * rc.y + wi[4] * rc.z + wi[5] * rc.w,
+                                       wi[6] * rc.y + wi[7] * rc.z + wi[8] * rc.w);
+        const float3 dnc = make_float3(wi[0] * dnrm.x + wi[1] * dnrm.y + wi[2] * dnrm.z, wi[3] * dnrm.x + wi[4] * dnrm.y + wi[5] * dnrm.z,
+                                       wi[6] * dnrm.x + wi[7] * dnrm.y + wi[8] * dnrm.z);
+        const float vx = dt.x + dpc.x, vy = dt.y + dpc.y, vz = dt.z + dpc.z;
+        const float J00 = hx * tz, J02 = -(hx * t.x) * tz2, J11 = hy * tz, J12 = -(hy * t.y) * tz2;
+        float n[3] = {0.f, 0.f, 0.f};  // world surfel normal: column argmin(scale) of R(q); none under cov3D_precomp
+        if (has_sr) {
+            const int axis = arg_min3(sc.x, sc.y, sc.z);
+#pragma unroll
+            for (int j = 0; j < 3; j++) n[j] = axis == 0 ? R[j][0] : (axis == 1 ? R[j][1] : R[j][2]);
+        }
+        const float mt[3] = {mean.x, mean.y, mean.z};
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            cam[3 * j + 0] = mt[j] * vx + J00 * dA0[j] + n[j] * dnc.x;
+            cam[3 * j + 1] = mt[j] * vy + J11 * dA1[j] + n[j] * dnc.y;
+            cam[3 * j + 2] = mt[j] * vz + J02 * dA0[j] + J12 * dA1[j] + n[j] * dnc.z;
+        }
+        cam[9] = vx; cam[10] = vy; cam[11] = vz;
+        // projection path: pixel = f(clip.xy / clip.w) with clip = P^T (mean, 1); dL/dclip from dL/dmean2D (g2x, g2y)
+        const float4 mh = xform4x4(mean, pj);
+        const float mw = 1.0f / (mh.w + 0.0000001f);
+        const float dcx = g2x * mw, dcy = g2y * mw, dcw = -(mh.x * g2x + mh.y * g2y) * mw * mw;
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            cam[12 + 3 * j] = mt[j] * dcx; cam[13 + 3 * j] = mt[j] * dcy; cam[14 + 3 * j] = mt[j] * dcw;
+        }
+        cam[21] = dcx; cam[22] = dcy; cam[23] = dcw;
+    }
+
     dL_dmeans[i3] = dmean.x; dL_dmeans[i3 + 1] = dmean.y; dL_dmeans[i3 + 2] = dmean.z;
     dL_dopacity[idx] = dopac;
     if (dL_dcolors) { dL_dcolors[i3] = dcol[0]; dL_dcolors[i3 + 1] = dcol[1]; dL_dcolors[i3 + 2] = dcol[2]; }
@@ -658,7 +705,85 @@ __global__ void __launch_bounds__(PBWD_THREADS, PBWD_MIN_BLOCKS) preprocess_bwd_
     __syncthreads();
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t V = *vis_count;
-    if ((uint32_t)idx < V) bwd_visible(vp, (int)g.vis_list[idx], M, s_m, means, scales, rots, shs, cov3D_precomp, g, rec, o);
+    if ((uint32_t)idx < V) bwd_visible<false>(vp, (int)g.vis_list[idx], M, s_m, means, scales, rots, shs, cov3D_precomp, g, rec, o, nullptr);
+}
+
+// The same backward that also returns dL/d(viewmatrix, projmatrix, campos): every visible Gaussian's RTG_CAM_TERMS terms
+// are summed by a warp butterfly, the block's eight warp sums in double in warp order, and the block partial goes to
+// `cam_partial` (double[RTG_CAM_TERMS] per block that holds a visible Gaussian); camera_grad_final_kernel adds the block
+// partials in block order. Nothing depends on timing, so identical records give a bit-identical camera gradient.
+__global__ void __launch_bounds__(PBWD_THREADS, PBWD_MIN_BLOCKS) preprocess_bwd_camera_kernel(const ViewParams vp, const int P, const int M,
+                                                                const float *__restrict__ means, const float *__restrict__ scales,
+                                                                const float *__restrict__ rots, const float *__restrict__ shs,
+                                                                const float *__restrict__ cov3D_precomp, const GeomState g,
+                                                                const uint32_t *__restrict__ vis_count, float *__restrict__ rec,
+                                                                const BwdOut o, double *__restrict__ cam_partial) {
+    __shared__ float s_m[48];
+    __shared__ float s_red[PBWD_THREADS / 32][RTG_CAM_TERMS];
+    if (threadIdx.x < 16) s_m[threadIdx.x] = vp.view[threadIdx.x];
+    else if (threadIdx.x < 32) s_m[threadIdx.x] = vp.proj[threadIdx.x - 16];
+    else if (threadIdx.x < 35) s_m[threadIdx.x] = vp.campos[threadIdx.x - 32];
+    __syncthreads();
+    if (threadIdx.x == 0) {  // W^-T = cofactor matrix / det of the 3x3 block W[i][k] = view[i + 4k]
+        const float *v = s_m;
+#define W_(i, k) v[(i) + 4 * (k)]
+        const float c00 = W_(1, 1) * W_(2, 2) - W_(1, 2) * W_(2, 1), c01 = W_(1, 2) * W_(2, 0) - W_(1, 0) * W_(2, 2),
+                    c02 = W_(1, 0) * W_(2, 1) - W_(1, 1) * W_(2, 0);
+        const float c10 = W_(0, 2) * W_(2, 1) - W_(0, 1) * W_(2, 2), c11 = W_(0, 0) * W_(2, 2) - W_(0, 2) * W_(2, 0),
+                    c12 = W_(0, 1) * W_(2, 0) - W_(0, 0) * W_(2, 1);
+        const float c20 = W_(0, 1) * W_(1, 2) - W_(0, 2) * W_(1, 1), c21 = W_(0, 2) * W_(1, 0) - W_(0, 0) * W_(1, 2),
+                    c22 = W_(0, 0) * W_(1, 1) - W_(0, 1) * W_(1, 0);
+        const float inv_det = 1.f / (W_(0, 0) * c00 + W_(0, 1) * c01 + W_(0, 2) * c02);
+#undef W_
+        const float c[9] = {c00, c01, c02, c10, c11, c12, c20, c21, c22};
+#pragma unroll
+        for (int i = 0; i < 9; i++) s_m[36 + i] = c[i] * inv_det;
+    }
+    __syncthreads();
+    const uint32_t V = *vis_count;
+    if ((uint32_t)blockIdx.x * blockDim.x >= V) return;  // block-uniform: no visible Gaussian, no partial
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    float cam[RTG_CAM_TERMS];
+#pragma unroll
+    for (int i = 0; i < RTG_CAM_TERMS; i++) cam[i] = 0.f;
+    if ((uint32_t)idx < V) bwd_visible<true>(vp, (int)g.vis_list[idx], M, s_m, means, scales, rots, shs, cov3D_precomp, g, rec, o, cam);
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+    for (int i = 0; i < RTG_CAM_TERMS; i++) {
+        float v = cam[i];
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+        if (lane == 0) s_red[w][i] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < RTG_CAM_TERMS) {
+        double acc = 0.0;
+#pragma unroll
+        for (int k = 0; k < PBWD_THREADS / 32; k++) acc += (double)s_red[k][threadIdx.x];
+        cam_partial[(size_t)blockIdx.x * RTG_CAM_TERMS + threadIdx.x] = acc;
+    }
+}
+
+// One warp per camera term: a fixed-stride double sum over the block partials, a fixed butterfly, one float store. Writes
+// all 35 outputs (view 16, proj 16, campos 3), the never-read entries as exact zeros.
+__global__ void __launch_bounds__(RTG_CAM_TERMS * 32) camera_grad_final_kernel(const uint32_t *__restrict__ vis_count,
+                                                                              const double *__restrict__ cam_partial,
+                                                                              float *__restrict__ dL_dcamera) {
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t nb = (*vis_count + PBWD_THREADS - 1) / PBWD_THREADS;
+    double acc = 0.0;
+    for (uint32_t b = lane; b < nb; b += 32) acc += cam_partial[(size_t)b * RTG_CAM_TERMS + w];
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+    if (lane == 0) {
+        int slot;
+        if (w < 12) slot = 4 * (w / 3) + w % 3;                                    // viewmatrix
+        else if (w < 24) slot = 16 + 4 * ((w - 12) / 3) + ((w - 12) % 3 == 2 ? 3 : (w - 12) % 3);  // projmatrix
+        else slot = 32 + (w - 24);                                                 // campos
+        dL_dcamera[slot] = (float)acc;
+    }
+    if (threadIdx.x < 4) dL_dcamera[4 * threadIdx.x + 3] = 0.f;
+    else if (threadIdx.x < 8) dL_dcamera[16 + 4 * (threadIdx.x - 4) + 2] = 0.f;
 }
 
 // ------------------------------------------------------------------ launchers
@@ -695,6 +820,26 @@ void launch_preprocess_bwd(const ViewParams &vp, int P, int M, const float *mean
     ProfScope ps(K_PREPROCESS_BWD, s);
     BwdOut o{dL_dmeans, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drot, dL_dcov3D, dL_dmeans2D};
     preprocess_bwd_kernel<<<(P + PBWD_THREADS - 1) / PBWD_THREADS, PBWD_THREADS, 0, s>>>(vp, P, M, means, scales, rots, shs, cov3D_precomp, g, vis_count, rec, o);
+}
+
+size_t camera_scratch_bytes(int P) {
+    const size_t blocks = P > 0 ? (size_t)(P + PBWD_THREADS - 1) / PBWD_THREADS : 1;
+    return blocks * RTG_CAM_TERMS * sizeof(double);
+}
+
+void launch_preprocess_bwd_camera(const ViewParams &vp, int P, int M, const float *means, const float *scales, const float *rots,
+                                  const float *shs, const float *cov3D_precomp, const GeomState &g, const uint32_t *vis_count,
+                                  float *rec, float *dL_dmeans, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
+                                  float *dL_dscales, float *dL_drot, float *dL_dcov3D, float *dL_dmeans2D, float *dL_dcamera,
+                                  void *camera_scratch, cudaStream_t s) {
+    if (P <= 0) return;
+    ProfScope ps(K_PREPROCESS_BWD, s);
+    BwdOut o{dL_dmeans, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drot, dL_dcov3D, dL_dmeans2D};
+    double *partial = reinterpret_cast<double *>(camera_scratch);
+    preprocess_bwd_camera_kernel<<<(P + PBWD_THREADS - 1) / PBWD_THREADS, PBWD_THREADS, 0, s>>>(vp, P, M, means, scales, rots, shs,
+                                                                                                cov3D_precomp, g, vis_count, rec, o,
+                                                                                                partial);
+    camera_grad_final_kernel<<<1, RTG_CAM_TERMS * 32, 0, s>>>(vis_count, partial, dL_dcamera);
 }
 
 }  // namespace rtg

@@ -284,14 +284,19 @@ def _forward_native(rs, means3D, sh, colors_precomp, opacities, scales, rotation
 
 
 class _RasterizeGaussians(torch.autograd.Function):
+    """The three trailing inputs are the settings' own viewmatrix / projmatrix / campos tensors, passed only when one of them
+    requires grad (rasterize_gaussians): autograd then asks for their gradients through ctx.needs_input_grad."""
+
     @staticmethod
-    def forward(ctx, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, tile_mask, raster_settings):
+    def forward(ctx, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, tile_mask, raster_settings,
+                viewmatrix=None, projmatrix=None, campos=None):
         outs, saved, inputs = _forward_native(raster_settings, means3D, sh, colors_precomp, opacities, scales, rotations,
                                               cov3Ds_precomp, tile_mask)
         color, depth, hit_color, hit_depth, hit_cw, hit_dw, T_map, radii = outs
         ctx.raster_settings = raster_settings
         ctx.native = saved
         ctx.provided = tuple(x is not None for x in inputs)
+        ctx.camera_shapes = tuple(None if t is None else t.shape for t in (viewmatrix, projmatrix, campos))
         e = torch.empty(0, device=means3D.device)
         ctx.save_for_backward(*[x if x is not None else e for x in inputs], radii, hit_depth, T_map)
         ctx.mark_non_differentiable(hit_color, hit_depth, radii)
@@ -352,14 +357,23 @@ class _RasterizeGaussians(torch.autograd.Function):
             raise RuntimeError(f"rasterizer: this frame needed {saved.pending.num_rendered} (Gaussian, tile) instances but its "
                                f"binning buffer held {saved.pending.r_cap}; it was rendered empty. The capacity has been raised: "
                                "render it again (set_capacity_checks('sync') makes every forward check its own count).")
+        camera = any(ctx.needs_input_grad[9:])  # only present when rasterize_gaussians passed the camera tensors
+        hook = _GRAD_RECORD_HOOK[0]
+        if camera and hook is not None:
+            raise RuntimeError("rasterizer: camera gradients (viewmatrix / projmatrix / campos with requires_grad) are not "
+                               "available with a gradient-record exchange hook (set_grad_record_hook, tile-sharded frames)")
+        g_cam = torch.zeros((35,), **f32) if camera else None  # (view 16, proj 16, campos 3); stays 0 for P == 0
         if P > 0:
             args = (C.byref(view), P, M, _ptr(means3D), _ptr(sh), _ptr(colors_precomp), _ptr(scales), _ptr(rotations),
                     _ptr(cov3Ds_precomp), _ptr(radii), C.c_void_p(saved.geom), C.c_void_p(saved.img), C.c_void_p(saved.bin), saved.r_cap,
                     C.c_void_p(saved.counters), _ptr(T_map), _ptr(hit_depth), _ptr(grad_out_color), _ptr(grad_out_depth), _ptr(scratch),
                     _ptr(g_means), _ptr(g_sh), _ptr(g_colors), _ptr(g_opac), _ptr(g_scales), _ptr(g_rot), _ptr(g_cov), None,
                     C.c_void_p(stream))
-            hook = _GRAD_RECORD_HOOK[0]
-            if hook is None and _VISIBLE_ROWS_ONLY[0]:
+            if camera:
+                cam_scratch = torch.empty((int(L.rtg_splat_camera_scratch_bytes(P)),), dtype=torch.uint8, device=device)
+                check(L.rtg_splat_backward_camera(*args[:-1], 1 if _VISIBLE_ROWS_ONLY[0] else 0, _ptr(g_cam), _ptr(cam_scratch),
+                                                  args[-1]), "rtg_splat_backward_camera")
+            elif hook is None and _VISIBLE_ROWS_ONLY[0]:
                 check(L.rtg_splat_backward_visible(*args), "rtg_splat_backward_visible")
             elif hook is None:
                 check(L.rtg_splat_backward(*args), "rtg_splat_backward")
@@ -369,7 +383,11 @@ class _RasterizeGaussians(torch.autograd.Function):
                 hook(scratch[:P * 16].view(P, 16))
                 check(L.rtg_splat_backward_finish(*args), "rtg_splat_backward_finish")
         # same order as the forward's arguments (reference __init__.py:269-279)
-        return g_means, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov, None, None
+        grads = (g_means, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov, None, None)
+        if len(ctx.needs_input_grad) == 9:
+            return grads
+        cam = (slice(0, 16), slice(16, 32), slice(32, 35))
+        return grads + tuple(g_cam[c].reshape(s) if n else None for c, s, n in zip(cam, ctx.camera_shapes, ctx.needs_input_grad[9:]))
 
 
 # Optional destination of the dense gradients (see `grad_buffers`); None = allocate per call.
@@ -430,6 +448,12 @@ def set_grad_record_hook(fn):
 
 
 def rasterize_gaussians(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, tile_mask, raster_settings):
+    """With grad mode on and any of raster_settings.viewmatrix / projmatrix / campos requiring grad, the backward also
+    returns their gradients (dL/d of each tensor as stored, rtg_splat_backward_camera); otherwise they are constants."""
+    cam = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in cam):
+        return _RasterizeGaussians.apply(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, tile_mask,
+                                         raster_settings, *cam)
     return _RasterizeGaussians.apply(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, tile_mask,
                                      raster_settings)
 

@@ -235,6 +235,44 @@ int rtg_splat_backward_render_dt(int32_t p_begin, int32_t p_end, const RtgSplatV
                                  float *dL_dcolors_precomp, float *dL_dopacity, float *dL_dscales, float *dL_drotations,
                                  float *dL_dcov3D, float *dL_dmeans2D, void *stream);
 
+/* ---- pose refinement against a frozen map (no reference counterpart) -----------------------------------------------
+ * rtg_splat_backward_pose: rtg_splat_backward_dt's camera gradient without any per-Gaussian gradient, for a loss in which
+ * only the camera is optimised. Same arguments minus the eight per-Gaussian outputs and visible_rows_only; dL_dT may be
+ * NULL; dL_dcamera (35 floats, all written) and camera_scratch as in rtg_splat_backward_camera, both required. The
+ * compositing backward is the same; the per-Gaussian pass computes only the camera terms, stores nothing per Gaussian
+ * and needs no zero fill. `grad2d_scratch` is all-zero on entry and left all-zero, as in every backward. Identical
+ * gradient records give a bit-identical dL_dcamera (fixed-order reduction). Validates on the host before any CUDA work. */
+int rtg_splat_backward_pose(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                            const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                            const int32_t *radii, const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap,
+                            const int32_t *counters, const float *final_T, const int32_t *hit_image, const float *dL_dcolor,
+                            const float *dL_ddepth, const float *dL_dT, float *grad2d_scratch, float *dL_dcamera,
+                            void *camera_scratch, void *stream);
+
+/* rtg_pose_adam_step: one Adam step of a camera pose on the device, from the camera gradients of the last backward. The
+ * pose is W2C (world to camera, row-major 4x4, double, kept on the device so that hundreds of steps do not drift it off
+ * SE(3)); the rasterizer reads viewmatrix = W2C^T, projmatrix = viewmatrix @ projection (`projection`: the camera's
+ * projection_matrix as stored, 16 floats) and campos = -R^T t. The step
+ *   1. collects G = dL/dW2C through those three arrays and the gradient of the left twist xi = (rho, phi) at zero,
+ *      W2C(xi) = exp(xi^) W2C: with A = G W2C^T, dL/drho_k = A[k][3], dL/dphi = (A21 - A12, A02 - A20, A10 - A01);
+ *   2. takes one bias-corrected Adam step on that 6-vector from xi = 0 (torch.optim.Adam's update: lr_trans for rho,
+ *      lr_rot for phi, `step` >= 1 counted by the caller as in rtg_adam_step), moments exp_avg / exp_avg_sq (6 floats
+ *      each, rho then phi) carried across calls;
+ *   3. applies W2C <- exp(xi^) W2C with the closed-form SE(3) exponential, resets xi to zero, and rewrites viewmatrix,
+ *      projmatrix and campos in place from the double pose.
+ * A NULL gradient pointer counts as zero. One single-block launch; validates on the host before any CUDA work. */
+typedef struct RtgPoseAdam {
+    double *pose;                                                  /* 16, W2C row-major, updated in place */
+    float *exp_avg, *exp_avg_sq;                                   /* 6 each */
+    const float *dL_dviewmatrix, *dL_dprojmatrix, *dL_dcampos;     /* 16, 16, 3 (rtg_splat_backward_camera's layout) */
+    const float *projection;                                       /* 16 */
+    float *viewmatrix, *projmatrix, *campos;                       /* 16, 16, 3: written */
+    float lr_trans, lr_rot;
+    float beta1, beta2, eps;
+    int32_t step;
+} RtgPoseAdam;
+int rtg_pose_adam_step(const RtgPoseAdam *s, void *stream);
+
 /* Replaces CudaRasterizer::Rasterizer::markVisible (rasterizer.h:21-26, rasterizer_impl.cu:145-157). */
 int rtg_splat_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix,
                            uint8_t *present, void *stream);

@@ -57,6 +57,14 @@ class RtgHistoryMerge(C.Structure):
                 + [(n, C.c_int32) for n in ("features_dc_stride", "features_rest_stride", "features_rest_width", "_pad")])
 
 
+class RtgPoseAdam(C.Structure):
+    """include/rtg_splat_b200.h: RtgPoseAdam (field order is the ABI)."""
+    _fields_ = ([(n, C.c_void_p) for n in ("pose", "exp_avg", "exp_avg_sq", "dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos",
+                                           "projection", "viewmatrix", "projmatrix", "campos")]
+                + [(n, C.c_float) for n in ("lr_trans", "lr_rot", "beta1", "beta2", "eps")]
+                + [("step", C.c_int32)])
+
+
 class RtgIcpLevel(C.Structure):
     _fields_ = [("vertex0", C.c_void_p), ("normal0", C.c_void_p), ("vertex1", C.c_void_p), ("normal1", C.c_void_p),
                 ("H", C.c_int32), ("W", C.c_int32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
@@ -85,6 +93,9 @@ SIGNATURES = {
     # _BWD_ARGS with dL_dT after dL_ddepth (argument 19)
     "rtg_splat_backward_dt": (C.c_int, _BWD_ARGS[:19] + [_VP] + _BWD_ARGS[19:-1] + [_I32, _VP, _VP, _VP]),
     "rtg_splat_backward_render_dt": (C.c_int, [_I32, _I32] + _BWD_ARGS[:19] + [_VP] + _BWD_ARGS[19:]),
+    # rtg_splat_backward_dt's arguments up to grad2d_scratch, then dL_dcamera, camera_scratch, stream
+    "rtg_splat_backward_pose": (C.c_int, _BWD_ARGS[:19] + [_VP, _VP] + [_VP, _VP, _VP]),
+    "rtg_pose_adam_step": (C.c_int, [C.POINTER(RtgPoseAdam), _VP]),
     "rtg_splat_mark_visible": (C.c_int, [_I32, _VP, _VP, _VP, _VP, _VP]),
     "rtg_adam_step": (C.c_int, [C.POINTER(RtgAdamGroup), _I32, _F, _F, _F, _I32, _VP]),
     "rtg_map_adam_step": (C.c_int, [C.POINTER(RtgMapStep), _VP]),

@@ -77,4 +77,113 @@ int launch_adam(const RtgAdamGroup *groups, int n_groups, float beta1, float bet
     return 0;
 }
 
+// ------------------------------------------------------------------ pose step (rtg_pose_adam_step)
+// A few hundred double operations with a chain of dependencies: one thread does them all. Not bracketed by the event
+// profiler: its ids are fixed, and timing it under `adam` would mix pose steps into the map optimizer's entry.
+__global__ void __launch_bounds__(1) pose_adam_kernel(const RtgPoseAdam s, const double bc1, const double bc2_sqrt) {
+    double T[4][4];
+#pragma unroll
+    for (int i = 0; i < 16; i++) T[i / 4][i % 4] = s.pose[i];
+
+    // G = dL/dW2C through viewmatrix = W2C^T, projmatrix = W2C^T @ projection and campos = -R^T t
+    double G[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            double v = s.dL_dviewmatrix ? (double)s.dL_dviewmatrix[4 * j + i] : 0.0;
+            if (s.dL_dprojmatrix)
+#pragma unroll
+                for (int k = 0; k < 4; k++) v += (double)s.projection[4 * i + k] * (double)s.dL_dprojmatrix[4 * j + k];
+            G[i][j] = v;
+        }
+    if (s.dL_dcampos) {
+        const double gc[3] = {s.dL_dcampos[0], s.dL_dcampos[1], s.dL_dcampos[2]};
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+#pragma unroll
+            for (int i = 0; i < 3; i++) G[k][i] -= T[k][3] * gc[i];
+            G[k][3] -= T[k][0] * gc[0] + T[k][1] * gc[1] + T[k][2] * gc[2];
+        }
+    }
+    // tangent gradient of the left twist at zero: A = G W2C^T
+    double A[3][4];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int k = 0; k < 4; k++) A[i][k] = G[i][0] * T[k][0] + G[i][1] * T[k][1] + G[i][2] * T[k][2] + G[i][3] * T[k][3];
+    const double grad[6] = {A[0][3], A[1][3], A[2][3], A[2][1] - A[1][2], A[0][2] - A[2][0], A[1][0] - A[0][1]};
+
+    // Adam from xi = 0 (torch.optim.Adam, _single_tensor_adam): xi = -lr / bc1 * m / (sqrt(v) / sqrt(bc2) + eps)
+    const double b1 = s.beta1, b2 = s.beta2;
+    double xi[6];
+#pragma unroll
+    for (int k = 0; k < 6; k++) {
+        const double m = b1 * (double)s.exp_avg[k] + (1.0 - b1) * grad[k];
+        const double v = b2 * (double)s.exp_avg_sq[k] + (1.0 - b2) * grad[k] * grad[k];
+        s.exp_avg[k] = (float)m;
+        s.exp_avg_sq[k] = (float)v;
+        const double lr = k < 3 ? s.lr_trans : s.lr_rot;
+        xi[k] = -(lr / bc1) * m / (sqrt(v) / bc2_sqrt + (double)s.eps);
+    }
+
+    // exp(xi^) = [[R, V rho], [0, 1]], R = I + a K + b K^2, V = I + b K + c K^2, K = [phi]x
+    const double p0 = xi[3], p1 = xi[4], p2 = xi[5];
+    const double th2 = p0 * p0 + p1 * p1 + p2 * p2;
+    double a, b, c;
+    if (th2 < 1e-4) {  // Taylor series; the first omitted terms are below 1e-16
+        a = 1.0 - th2 / 6.0 * (1.0 - th2 / 20.0);
+        b = 0.5 - th2 / 24.0 * (1.0 - th2 / 30.0);
+        c = 1.0 / 6.0 - th2 / 120.0 * (1.0 - th2 / 42.0);
+    } else {
+        const double th = sqrt(th2), sn = sin(th), cs = cos(th);
+        a = sn / th;
+        b = (1.0 - cs) / th2;
+        c = (th - sn) / (th2 * th);
+    }
+    const double K[3][3] = {{0.0, -p2, p1}, {p2, 0.0, -p0}, {-p1, p0, 0.0}};
+    double E[3][4];
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+        double Vr = 0.0;
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            const double K2 = K[i][0] * K[0][j] + K[i][1] * K[1][j] + K[i][2] * K[2][j];
+            const double I = i == j ? 1.0 : 0.0;
+            E[i][j] = I + a * K[i][j] + b * K2;
+            Vr += (I + b * K[i][j] + c * K2) * xi[j];
+        }
+        E[i][3] = Vr;
+    }
+    double N[4][4];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) N[i][j] = E[i][0] * T[0][j] + E[i][1] * T[1][j] + E[i][2] * T[2][j] + (j == 3 ? E[i][3] : 0.0);
+#pragma unroll
+    for (int j = 0; j < 4; j++) N[3][j] = T[3][j];
+
+#pragma unroll
+    for (int i = 0; i < 16; i++) s.pose[i] = N[i / 4][i % 4];
+#pragma unroll
+    for (int r = 0; r < 4; r++)
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+            s.viewmatrix[4 * r + q] = (float)N[q][r];
+            double pm = 0.0;
+#pragma unroll
+            for (int k = 0; k < 4; k++) pm += N[k][r] * (double)s.projection[4 * k + q];
+            s.projmatrix[4 * r + q] = (float)pm;
+        }
+#pragma unroll
+    for (int i = 0; i < 3; i++) s.campos[i] = (float)-(N[0][i] * N[0][3] + N[1][i] * N[1][3] + N[2][i] * N[2][3]);
+}
+
+void launch_pose_adam_step(const RtgPoseAdam &st, cudaStream_t s) {
+    // bias corrections in double, as rtg_adam_step (torch computes them in python floats)
+    const double bc1 = 1.0 - pow((double)st.beta1, (double)st.step);
+    const double bc2_sqrt = sqrt(1.0 - pow((double)st.beta2, (double)st.step));
+    pose_adam_kernel<<<1, 1, 0, s>>>(st, bc1, bc2_sqrt);
+}
+
 }  // namespace rtg

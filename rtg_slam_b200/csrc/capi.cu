@@ -14,6 +14,7 @@
 
 namespace rtg {
 int launch_adam(const RtgAdamGroup *groups, int n_groups, float beta1, float beta2, float eps, int step, cudaStream_t s);
+void launch_pose_adam_step(const RtgPoseAdam &st, cudaStream_t s);
 void launch_map_adam_step(const RtgMapStep &st, cudaStream_t s);
 void launch_history_merge(const RtgHistoryMerge &m, cudaStream_t s);
 void launch_map_activate(int P, const float *scaling_raw, const float *rotation_raw, const float *opacity_raw, float *scales_out,
@@ -471,6 +472,60 @@ int rtg_splat_backward_render_dt(int32_t p_begin, int32_t p_end, RTG_BWD_DT_PARA
     if (rc) return rc;
     if (p_begin < 0 || p_end < p_begin || p_end > P) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_splat_backward_render_dt: bad range");
     return splat_backward_impl(1, p_begin, p_end, RTG_BWD_ARGS, nullptr, nullptr, dL_dT);
+}
+
+int rtg_splat_backward_pose(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                            const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                            const int32_t *radii, const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap,
+                            const int32_t *counters, const float *final_T, const int32_t *hit_image, const float *dL_dcolor,
+                            const float *dL_ddepth, const float *dL_dT, float *grad2d_scratch, float *dL_dcamera,
+                            void *camera_scratch, void *stream) {
+    const char *who = "rtg_splat_backward_pose";
+    int rc = validate_dT(who, view, P, dL_dT);
+    if (rc) return rc;
+    if (!dL_dcamera || !camera_scratch)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": dL_dcamera / camera_scratch is NULL");
+    if (((uintptr_t)camera_scratch) & 7)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": camera_scratch must be 8-byte aligned");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    if (P == 0) {  // nothing visible: the camera gradient is zero
+        cudaError_t e = cudaMemsetAsync(dL_dcamera, 0, 35 * sizeof(float), s);
+        if (e != cudaSuccess) return fail(RTG_ERR_CUDA, std::string(who) + " memset: " + cudaGetErrorString(e));
+        return RTG_OK;
+    }
+    if (!means3D || !radii || !geom_ws || !img_ws || !bin_ws || !counters || !final_T || !hit_image || !dL_dcolor || !dL_ddepth ||
+        !grad2d_scratch)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pointer");
+    if ((shs == nullptr) == (colors_precomp == nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "Please provide excatly one of either SHs or precomputed colors!");
+    if (((scales == nullptr || rotations == nullptr) && cov3D_precomp == nullptr) ||
+        ((scales != nullptr || rotations != nullptr) && cov3D_precomp != nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
+    if (shs && (M < (view->sh_degree + 1) * (view->sh_degree + 1) || M > 16))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": M must hold (sh_degree+1)^2 coefficients and be <= 16");
+    if ((((uintptr_t)grad2d_scratch) & 15) || (((uintptr_t)rotations) & 15) || (M == 16 && (((uintptr_t)shs) & 15)))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": grad2d_scratch / rotations / shs must be 16-byte aligned");
+    const rtg::ViewParams vp = make_view(view);
+    const int T = vp.tiles_x * vp.tiles_y;
+    rtg::GeomState g = rtg::geom_from(const_cast<void *>(geom_ws), (size_t)P);
+    rtg::ImgState img = rtg::img_from(const_cast<void *>(img_ws), (size_t)vp.H * vp.W);
+    rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
+    rtg::launch_render_bwd(vp, g, b, img, counters, final_T, hit_image, dL_dcolor, dL_ddepth, grad2d_scratch, s, dL_dT);
+    rtg::launch_preprocess_bwd_pose(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count, grad2d_scratch,
+                                    dL_dcamera, camera_scratch, s);
+    return check_launch(who);
+}
+
+int rtg_pose_adam_step(const RtgPoseAdam *st, void *stream) {
+    if (!st) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_pose_adam_step: state is NULL");
+    if (!st->pose || !st->exp_avg || !st->exp_avg_sq)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_pose_adam_step: NULL pose / exp_avg / exp_avg_sq");
+    if (!st->projection || !st->viewmatrix || !st->projmatrix || !st->campos)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_pose_adam_step: NULL projection / viewmatrix / projmatrix / campos");
+    if (((uintptr_t)st->pose) & 7) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_pose_adam_step: pose must be 8-byte aligned");
+    if (st->step < 1) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_pose_adam_step: step must be >= 1");
+    rtg::launch_pose_adam_step(*st, reinterpret_cast<cudaStream_t>(stream));
+    return check_launch("rtg_pose_adam_step");
 }
 
 int rtg_splat_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix, uint8_t *present,

@@ -24,6 +24,10 @@ void launch_preprocess_bwd_camera(const ViewParams &vp, int P, int M, const floa
                                   float *rec, float *dL_dmeans, float *dL_dsh, float *dL_dcolors, float *dL_dopacity,
                                   float *dL_dscales, float *dL_drot, float *dL_dcov3D, float *dL_dmeans2D, float *dL_dcamera,
                                   void *camera_scratch, cudaStream_t s);
+// the camera gradient alone (frozen map): the records are consumed and cleared, no per-Gaussian gradient is written
+void launch_preprocess_bwd_pose(const ViewParams &vp, int P, int M, const float *means, const float *scales, const float *rots,
+                                const float *shs, const float *cov3D_precomp, const GeomState &g, const uint32_t *vis_count,
+                                float *rec, float *dL_dcamera, void *camera_scratch, cudaStream_t s);
 
 // binning.cu
 void launch_tile_histogram(const ViewParams &vp, int P, const GeomState &g, const int *radii, const int *tile_mask, const BinState &b,

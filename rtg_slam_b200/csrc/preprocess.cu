@@ -362,7 +362,9 @@ __device__ __forceinline__ void bwd_zero(const int idx, const int M, const bool 
 // SH part of the backward (computeColorFromSH, backward.cu:152-268): dL/dsh and the view-direction term of dL/dmean.
 // Inlined, with 128 registers per thread (2 CTAs / SM): the kernel is bound by memory latency, not by occupancy --
 // what pays is that all of a thread's independent loads (record, mean, scale, rotation, 12 x 16 B of SH) are in
-// flight together.
+// flight together. STORE_DSH = false is the store-free form of the pose-only backward: it returns the view-direction
+// term alone and leaves dL_dsh (then NULL) untouched.
+template <bool STORE_DSH = true>
 __device__ __forceinline__ float3 bwd_sh(const int deg, const int idx, const int M, const float3 mean, const float3 campos,
                                       const float dcol0, const float dcol1, const float dcol2, const int flags,
                                       const float *__restrict__ shs, float *__restrict__ dL_dsh) {
@@ -388,23 +390,25 @@ __device__ __forceinline__ float3 bwd_sh(const int deg, const int idx, const int
         w[14] = SH_C3_5 * z * (xx - yy); w[15] = SH_C3_6 * x * (xx - 3.f * yy);
         const int nc = sh_ncoef(deg);
         // dL/dsh[k][ch] = w[k] * dRGB[ch] for k < (deg+1)^2, zero above; constant indices only (keeps w[] in registers)
-        if (M == 16) {
-            float4 *o4 = reinterpret_cast<float4 *>(dL_dsh + (size_t)idx * 48);
+        if constexpr (STORE_DSH) {
+            if (M == 16) {
+                float4 *o4 = reinterpret_cast<float4 *>(dL_dsh + (size_t)idx * 48);
 #pragma unroll
-            for (int i = 0; i < 12; i++) {
-                float e[4];
+                for (int i = 0; i < 12; i++) {
+                    float e[4];
 #pragma unroll
-                for (int t = 0; t < 4; t++) {
-                    const int k = (4 * i + t) / 3, ch = (4 * i + t) % 3;
-                    e[t] = (k < nc) ? w[k] * dRGB[ch] : 0.f;
+                    for (int t = 0; t < 4; t++) {
+                        const int k = (4 * i + t) / 3, ch = (4 * i + t) % 3;
+                        e[t] = (k < nc) ? w[k] * dRGB[ch] : 0.f;
+                    }
+                    o4[i] = make_float4(e[0], e[1], e[2], e[3]);
                 }
-                o4[i] = make_float4(e[0], e[1], e[2], e[3]);
-            }
-        } else {
-            float *o1 = dL_dsh + (size_t)idx * 3 * M;
+            } else {
+                float *o1 = dL_dsh + (size_t)idx * 3 * M;
 #pragma unroll
-            for (int e = 0; e < 48; e++)
-                if (e < 3 * M) o1[e] = (e / 3 < nc) ? w[e / 3] * dRGB[e % 3] : 0.f;
+                for (int e = 0; e < 48; e++)
+                    if (e < 3 * M) o1[e] = (e / 3 < nc) ? w[e / 3] * dRGB[e % 3] : 0.f;
+            }
         }
         float3 ddir = make_float3(0.f, 0.f, 0.f);
 #pragma unroll
@@ -449,12 +453,18 @@ __device__ __forceinline__ float3 bwd_sh(const int deg, const int idx, const int
 //   [24+i]      i < 3          dL/dcampos[i]
 #define RTG_CAM_TERMS 27
 
-template <bool CAMERA>
+// What bwd_visible produces: the per-Gaussian gradients (BWD_GAUSSIAN), those and the camera terms (BWD_CAMERA), or the
+// camera terms alone (BWD_POSE: a frozen map, nothing per Gaussian is stored -- only the record is consumed and cleared).
+enum BwdMode { BWD_GAUSSIAN, BWD_CAMERA, BWD_POSE };
+
+template <int MODE>
 __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx, const int M, const float *s_m,
                                             const float *__restrict__ means, const float *__restrict__ scales,
                                             const float *__restrict__ rots, const float *__restrict__ shs,
                                             const float *__restrict__ cov3D_precomp, const GeomState &g, float *__restrict__ rec,
                                             const BwdOut &o, float *cam) {
+    constexpr bool CAMERA = MODE != BWD_GAUSSIAN;   // the camera terms go to cam[]
+    constexpr bool GAUSSIANS = MODE != BWD_POSE;    // the per-Gaussian gradients are stored
     const float *vm = s_m, *pj = s_m + 16;
     const size_t i3 = 3 * (size_t)idx;
     const bool has_sh = (shs != nullptr);
@@ -484,8 +494,8 @@ __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx,
 
     const float3 mean = make_float3(means[i3], means[i3 + 1], means[i3 + 2]);
     if (has_sh) {
-        const float3 dsh_mean = bwd_sh(vp.sh_degree, idx, M, mean, make_float3(s_m[32], s_m[33], s_m[34]), dcol[0], dcol[1], dcol[2],
-                                       __float_as_int(g.rgb_flags[idx].w), shs, dL_dsh);
+        const float3 dsh_mean = bwd_sh<GAUSSIANS>(vp.sh_degree, idx, M, mean, make_float3(s_m[32], s_m[33], s_m[34]), dcol[0], dcol[1],
+                                                  dcol[2], __float_as_int(g.rgb_flags[idx].w), shs, dL_dsh);
         dmean.x += dsh_mean.x; dmean.y += dsh_mean.y; dmean.z += dsh_mean.z;
         if constexpr (CAMERA) {  // campos enters only through the view direction mean - campos
             cam[24] = -dsh_mean.x; cam[25] = -dsh_mean.y; cam[26] = -dsh_mean.z;
@@ -500,26 +510,28 @@ __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx,
         q = reinterpret_cast<const float4 *>(rots)[idx];
         quat_to_R(q, R);
         cov3d_from(sc, vp.scale_modifier, R, c6);
-        // depth path: the surfel normal is column argmin(scale) of R(q); d(normal)/dq of propagateRotationGrad
-        // (backward.cu:100-148) applied to the accumulated dL/dnormal
-        const int axis = arg_min3(sc.x, sc.y, sc.z);
-        const float q0 = q.x, q1 = q.y, q2 = q.z, q3 = q.w;
-        const float w1 = dnrm.x, w2 = dnrm.y, w3 = dnrm.z;
-        if (axis == 0) {
-            drot.x = w2 * (2 * q3) + w3 * (-2 * q2);
-            drot.y = w2 * (2 * q2) + w3 * (2 * q3);
-            drot.z = w1 * (-4 * q2) + w2 * (2 * q1) + w3 * (-2 * q0);
-            drot.w = w1 * (-4 * q3) + w2 * (2 * q0) + w3 * (2 * q1);
-        } else if (axis == 1) {
-            drot.x = w1 * (-2 * q3) + w3 * (2 * q1);
-            drot.y = w1 * (2 * q2) + w2 * (-4 * q1) + w3 * (2 * q0);
-            drot.z = w1 * (2 * q1) + w3 * (2 * q3);
-            drot.w = w1 * (-2 * q0) + w2 * (-4 * q3) + w3 * (2 * q2);
-        } else {
-            drot.x = w1 * (2 * q2) + w2 * (-2 * q1);
-            drot.y = w1 * (2 * q3) + w2 * (-2 * q0) + w3 * (-4 * q1);
-            drot.z = w1 * (2 * q0) + w2 * (2 * q3) + w3 * (-4 * q2);
-            drot.w = w1 * (2 * q1) + w2 * (2 * q2);
+        if constexpr (GAUSSIANS) {
+            // depth path: the surfel normal is column argmin(scale) of R(q); d(normal)/dq of propagateRotationGrad
+            // (backward.cu:100-148) applied to the accumulated dL/dnormal
+            const int axis = arg_min3(sc.x, sc.y, sc.z);
+            const float q0 = q.x, q1 = q.y, q2 = q.z, q3 = q.w;
+            const float w1 = dnrm.x, w2 = dnrm.y, w3 = dnrm.z;
+            if (axis == 0) {
+                drot.x = w2 * (2 * q3) + w3 * (-2 * q2);
+                drot.y = w2 * (2 * q2) + w3 * (2 * q3);
+                drot.z = w1 * (-4 * q2) + w2 * (2 * q1) + w3 * (-2 * q0);
+                drot.w = w1 * (-4 * q3) + w2 * (2 * q0) + w3 * (2 * q1);
+            } else if (axis == 1) {
+                drot.x = w1 * (-2 * q3) + w3 * (2 * q1);
+                drot.y = w1 * (2 * q2) + w2 * (-4 * q1) + w3 * (2 * q0);
+                drot.z = w1 * (2 * q1) + w3 * (2 * q3);
+                drot.w = w1 * (-2 * q0) + w2 * (-4 * q3) + w3 * (2 * q2);
+            } else {
+                drot.x = w1 * (2 * q2) + w2 * (-2 * q1);
+                drot.y = w1 * (2 * q3) + w2 * (-2 * q0) + w3 * (-4 * q1);
+                drot.z = w1 * (2 * q0) + w2 * (2 * q3) + w3 * (-4 * q2);
+                drot.w = w1 * (2 * q1) + w2 * (2 * q2);
+            }
         }
     } else {
 #pragma unroll
@@ -542,12 +554,14 @@ __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx,
         da = denom2inv * (-c * c * dcon[0] + 2 * b * c * dcon[1] + (denom - a * c) * dcon[2]);
         dc = denom2inv * (-a * a * dcon[2] + 2 * a * b * dcon[1] + (denom - a * c) * dcon[0]);
         db = denom2inv * 2 * (b * c * dcon[0] - (denom + 2 * b * b) * dcon[1] + a * b * dcon[2]);
-        dcov[0] = A0[0] * A0[0] * da + A0[0] * A1[0] * db + A1[0] * A1[0] * dc;
-        dcov[3] = A0[1] * A0[1] * da + A0[1] * A1[1] * db + A1[1] * A1[1] * dc;
-        dcov[5] = A0[2] * A0[2] * da + A0[2] * A1[2] * db + A1[2] * A1[2] * dc;
-        dcov[1] = 2 * A0[0] * A0[1] * da + (A0[0] * A1[1] + A0[1] * A1[0]) * db + 2 * A1[0] * A1[1] * dc;
-        dcov[2] = 2 * A0[0] * A0[2] * da + (A0[0] * A1[2] + A0[2] * A1[0]) * db + 2 * A1[0] * A1[2] * dc;
-        dcov[4] = 2 * A0[2] * A0[1] * da + (A0[1] * A1[2] + A0[2] * A1[1]) * db + 2 * A1[1] * A1[2] * dc;
+        if constexpr (GAUSSIANS) {
+            dcov[0] = A0[0] * A0[0] * da + A0[0] * A1[0] * db + A1[0] * A1[0] * dc;
+            dcov[3] = A0[1] * A0[1] * da + A0[1] * A1[1] * db + A1[1] * A1[1] * dc;
+            dcov[5] = A0[2] * A0[2] * da + A0[2] * A1[2] * db + A1[2] * A1[2] * dc;
+            dcov[1] = 2 * A0[0] * A0[1] * da + (A0[0] * A1[1] + A0[1] * A1[0]) * db + 2 * A1[0] * A1[1] * dc;
+            dcov[2] = 2 * A0[0] * A0[2] * da + (A0[0] * A1[2] + A0[2] * A1[0]) * db + 2 * A1[0] * A1[2] * dc;
+            dcov[4] = 2 * A0[2] * A0[1] * da + (A0[1] * A1[2] + A0[2] * A1[1]) * db + 2 * A1[1] * A1[2] * dc;
+        }
     }
     float dA0[3], dA1[3];
 #pragma unroll
@@ -567,7 +581,7 @@ __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx,
     dmean.x += dm_cov.x; dmean.y += dm_cov.y; dmean.z += dm_cov.z;
 
     // ---- projection path, backward.cu:516-533
-    {
+    if constexpr (GAUSSIANS) {
         const float4 mh = xform4x4(mean, pj);
         const float mw = 1.0f / (mh.w + 0.0000001f);
         const float mul1 = (pj[0] * mean.x + pj[4] * mean.y + pj[8] * mean.z + pj[12]) * mw * mw;
@@ -580,7 +594,7 @@ __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx,
     // (SH path: bwd_sh, run first)
 
     // ---- cov3D -> scale, quaternion, backward.cu:426-487
-    if (has_sr) {
+    if (GAUSSIANS && has_sr) {
         const float sv[3] = {vp.scale_modifier * sc.x, vp.scale_modifier * sc.y, vp.scale_modifier * sc.z};
         float Mm[3][3], dS[3][3], dM[3][3], G[3][3];
 #pragma unroll
@@ -647,13 +661,15 @@ __device__ __forceinline__ void bwd_visible(const ViewParams &vp, const int idx,
         cam[21] = dcx; cam[22] = dcy; cam[23] = dcw;
     }
 
-    dL_dmeans[i3] = dmean.x; dL_dmeans[i3 + 1] = dmean.y; dL_dmeans[i3 + 2] = dmean.z;
-    dL_dopacity[idx] = dopac;
-    if (dL_dcolors) { dL_dcolors[i3] = dcol[0]; dL_dcolors[i3 + 1] = dcol[1]; dL_dcolors[i3 + 2] = dcol[2]; }
-    if (dL_dcov3D)
+    if constexpr (GAUSSIANS) {
+        dL_dmeans[i3] = dmean.x; dL_dmeans[i3 + 1] = dmean.y; dL_dmeans[i3 + 2] = dmean.z;
+        dL_dopacity[idx] = dopac;
+        if (dL_dcolors) { dL_dcolors[i3] = dcol[0]; dL_dcolors[i3 + 1] = dcol[1]; dL_dcolors[i3 + 2] = dcol[2]; }
+        if (dL_dcov3D)
 #pragma unroll
-        for (int i = 0; i < 6; i++) dL_dcov3D[6 * (size_t)idx + i] = dcov[i];
-    if (dL_dmeans2D) { dL_dmeans2D[i3] = g2x; dL_dmeans2D[i3 + 1] = g2y; dL_dmeans2D[i3 + 2] = 0.f; }
+            for (int i = 0; i < 6; i++) dL_dcov3D[6 * (size_t)idx + i] = dcov[i];
+        if (dL_dmeans2D) { dL_dmeans2D[i3] = g2x; dL_dmeans2D[i3 + 1] = g2y; dL_dmeans2D[i3 + 2] = 0.f; }
+    }
     {   // consume-and-clear: the record is cleared only now. A store to a line whose load is still in flight has to
         // wait for it, which would put one more memory round trip into every warp's life.
         const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -705,21 +721,21 @@ __global__ void __launch_bounds__(PBWD_THREADS, PBWD_MIN_BLOCKS) preprocess_bwd_
     __syncthreads();
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t V = *vis_count;
-    if ((uint32_t)idx < V) bwd_visible<false>(vp, (int)g.vis_list[idx], M, s_m, means, scales, rots, shs, cov3D_precomp, g, rec, o, nullptr);
+    if ((uint32_t)idx < V) bwd_visible<BWD_GAUSSIAN>(vp,(int)g.vis_list[idx], M, s_m, means, scales, rots, shs, cov3D_precomp, g, rec, o, nullptr);
 }
 
 // The same backward that also returns dL/d(viewmatrix, projmatrix, campos): every visible Gaussian's RTG_CAM_TERMS terms
 // are summed by a warp butterfly, the block's eight warp sums in double in warp order, and the block partial goes to
 // `cam_partial` (double[RTG_CAM_TERMS] per block that holds a visible Gaussian); camera_grad_final_kernel adds the block
 // partials in block order. Nothing depends on timing, so identical records give a bit-identical camera gradient.
-__global__ void __launch_bounds__(PBWD_THREADS, PBWD_MIN_BLOCKS) preprocess_bwd_camera_kernel(const ViewParams vp, const int P, const int M,
-                                                                const float *__restrict__ means, const float *__restrict__ scales,
-                                                                const float *__restrict__ rots, const float *__restrict__ shs,
-                                                                const float *__restrict__ cov3D_precomp, const GeomState g,
-                                                                const uint32_t *__restrict__ vis_count, float *__restrict__ rec,
-                                                                const BwdOut o, double *__restrict__ cam_partial) {
-    __shared__ float s_m[48];
-    __shared__ float s_red[PBWD_THREADS / 32][RTG_CAM_TERMS];
+// The body of the camera and the pose-only kernel; they own the shared arrays s_m[48] and s_red.
+template <int MODE>
+__device__ __forceinline__ void bwd_camera_block(float *s_m, float (*s_red)[RTG_CAM_TERMS], const ViewParams &vp, const int M,
+                                                 const float *__restrict__ means, const float *__restrict__ scales,
+                                                 const float *__restrict__ rots, const float *__restrict__ shs,
+                                                 const float *__restrict__ cov3D_precomp, const GeomState &g,
+                                                 const uint32_t *__restrict__ vis_count, float *__restrict__ rec, const BwdOut &o,
+                                                 double *__restrict__ cam_partial) {
     if (threadIdx.x < 16) s_m[threadIdx.x] = vp.view[threadIdx.x];
     else if (threadIdx.x < 32) s_m[threadIdx.x] = vp.proj[threadIdx.x - 16];
     else if (threadIdx.x < 35) s_m[threadIdx.x] = vp.campos[threadIdx.x - 32];
@@ -746,7 +762,7 @@ __global__ void __launch_bounds__(PBWD_THREADS, PBWD_MIN_BLOCKS) preprocess_bwd_
     float cam[RTG_CAM_TERMS];
 #pragma unroll
     for (int i = 0; i < RTG_CAM_TERMS; i++) cam[i] = 0.f;
-    if ((uint32_t)idx < V) bwd_visible<true>(vp, (int)g.vis_list[idx], M, s_m, means, scales, rots, shs, cov3D_precomp, g, rec, o, cam);
+    if ((uint32_t)idx < V) bwd_visible<MODE>(vp, (int)g.vis_list[idx], M, s_m, means, scales, rots, shs, cov3D_precomp, g, rec, o, cam);
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
 #pragma unroll
     for (int i = 0; i < RTG_CAM_TERMS; i++) {
@@ -762,6 +778,31 @@ __global__ void __launch_bounds__(PBWD_THREADS, PBWD_MIN_BLOCKS) preprocess_bwd_
         for (int k = 0; k < PBWD_THREADS / 32; k++) acc += (double)s_red[k][threadIdx.x];
         cam_partial[(size_t)blockIdx.x * RTG_CAM_TERMS + threadIdx.x] = acc;
     }
+}
+
+__global__ void __launch_bounds__(PBWD_THREADS, PBWD_MIN_BLOCKS) preprocess_bwd_camera_kernel(const ViewParams vp, const int P, const int M,
+                                                                const float *__restrict__ means, const float *__restrict__ scales,
+                                                                const float *__restrict__ rots, const float *__restrict__ shs,
+                                                                const float *__restrict__ cov3D_precomp, const GeomState g,
+                                                                const uint32_t *__restrict__ vis_count, float *__restrict__ rec,
+                                                                const BwdOut o, double *__restrict__ cam_partial) {
+    __shared__ float s_m[48];
+    __shared__ float s_red[PBWD_THREADS / 32][RTG_CAM_TERMS];
+    bwd_camera_block<BWD_CAMERA>(s_m, s_red, vp, M, means, scales, rots, shs, cov3D_precomp, g, vis_count, rec, o, cam_partial);
+}
+
+// Pose-only backward of a frozen map: the camera kernel's terms and reduction, with no per-Gaussian store (no SH, mean,
+// scale, rotation, opacity, colour or covariance gradient) -- each visible Gaussian's record is read and cleared.
+__global__ void __launch_bounds__(PBWD_THREADS, PBWD_MIN_BLOCKS) preprocess_bwd_pose_kernel(const ViewParams vp, const int M,
+                                                                const float *__restrict__ means, const float *__restrict__ scales,
+                                                                const float *__restrict__ rots, const float *__restrict__ shs,
+                                                                const float *__restrict__ cov3D_precomp, const GeomState g,
+                                                                const uint32_t *__restrict__ vis_count, float *__restrict__ rec,
+                                                                double *__restrict__ cam_partial) {
+    __shared__ float s_m[48];
+    __shared__ float s_red[PBWD_THREADS / 32][RTG_CAM_TERMS];
+    const BwdOut none{};
+    bwd_camera_block<BWD_POSE>(s_m, s_red, vp, M, means, scales, rots, shs, cov3D_precomp, g, vis_count, rec, none, cam_partial);
 }
 
 // One warp per camera term: a fixed-stride double sum over the block partials, a fixed butterfly, one float store. Writes
@@ -839,6 +880,18 @@ void launch_preprocess_bwd_camera(const ViewParams &vp, int P, int M, const floa
     preprocess_bwd_camera_kernel<<<(P + PBWD_THREADS - 1) / PBWD_THREADS, PBWD_THREADS, 0, s>>>(vp, P, M, means, scales, rots, shs,
                                                                                                 cov3D_precomp, g, vis_count, rec, o,
                                                                                                 partial);
+    camera_grad_final_kernel<<<1, RTG_CAM_TERMS * 32, 0, s>>>(vis_count, partial, dL_dcamera);
+}
+
+void launch_preprocess_bwd_pose(const ViewParams &vp, int P, int M, const float *means, const float *scales, const float *rots,
+                                const float *shs, const float *cov3D_precomp, const GeomState &g, const uint32_t *vis_count,
+                                float *rec, float *dL_dcamera, void *camera_scratch, cudaStream_t s) {
+    if (P <= 0) return;
+    ProfScope ps(K_PREPROCESS_BWD, s);
+    double *partial = reinterpret_cast<double *>(camera_scratch);
+    preprocess_bwd_pose_kernel<<<(P + PBWD_THREADS - 1) / PBWD_THREADS, PBWD_THREADS, 0, s>>>(vp, M, means, scales, rots, shs,
+                                                                                              cov3D_precomp, g, vis_count, rec,
+                                                                                              partial);
     camera_grad_final_kernel<<<1, RTG_CAM_TERMS * 32, 0, s>>>(vis_count, partial, dL_dcamera);
 }
 

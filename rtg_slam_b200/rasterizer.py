@@ -48,6 +48,11 @@ class GaussianRasterizationSettings(NamedTuple):
     T_threshold: float = 0.0001
 
 
+class CapacityOverflow(RuntimeError):
+    """A forward needed more (Gaussian, tile) instances than its binning buffer held and rendered that frame empty. The
+    capacity has been raised by the time this is raised: rendering the frame again succeeds."""
+
+
 # ----------------------------------------------------------------------------- per-device state
 class _Pending:
     """Counters of one forward call that have not been read yet: pinned buffer + the event recorded after the scan kernel."""
@@ -110,7 +115,7 @@ class _DeviceState:
             if self.read(p, block) and p.overflow:
                 bad = p
         if bad is not None:
-            raise RuntimeError(
+            raise CapacityOverflow(
                 f"rasterizer: an earlier forward needed {bad.num_rendered} (Gaussian, tile) instances but its binning buffer "
                 f"held {bad.r_cap}; that frame was rendered empty. The capacity has been raised -- render the frame again, "
                 "or call set_capacity_checks('sync') to have every forward wait for its own count.")
@@ -143,7 +148,7 @@ def set_capacity_checks(mode: str, device=None) -> None:
     'sync'     every forward waits for its scan kernel (not for the rest of the forward) and re-runs on overflow;
     'auto'     (default) the first forward of a (P, H, W) shape does that; later ones do not wait -- the buffer holds 1.5x
                the largest count seen, their counters are read once they have arrived, and an overflow (which leaves that
-               frame empty) raises RuntimeError at the next rasterizer call or at the frame's own backward;
+               frame empty) raises CapacityOverflow (a RuntimeError) at the next rasterizer call or at the frame's own backward;
     'deferred' like 'auto' without the waiting first call."""
     if mode not in ("sync", "auto", "deferred"):
         raise ValueError("mode must be 'sync', 'auto' or 'deferred'")
@@ -335,6 +340,12 @@ class _RasterizeGaussians(torch.autograd.Function):
         st = _state(device)
 
         buf = _GRAD_BUFFERS[0]
+        camera = any(ctx.needs_input_grad[9:])  # only present when rasterize_gaussians passed the camera tensors
+        hook = _GRAD_RECORD_HOOK[0]
+        # A frozen map (pose refinement): only the camera is differentiated. Autograd would discard per-Gaussian gradients
+        # here, so rtg_splat_backward_pose computes none of them.
+        pose_only = (camera and hook is None and buf is None and not _VISIBLE_ROWS_ONLY[0]
+                     and not any(ctx.needs_input_grad[:7]))
 
         def out(name, shape):
             """Gradient tensor: a fresh allocation, or -- inside `grad_buffers(...)` -- a fresh alias of the caller's buffer
@@ -347,22 +358,23 @@ class _RasterizeGaussians(torch.autograd.Function):
                     raise ValueError(f"grad buffer '{name}' must start at a 16-byte aligned address (the kernels store 128 bits at a time)")
                 return t.view(shape)
             return torch.empty(shape, **f32)
-        g_means = out("means3D", (P, 3))
-        g_opac = out("opacities", (P, 1))
-        g_sh = out("shs", (P, M, 3)) if sh is not None else None
-        g_colors = torch.empty((P, 3), **f32) if colors_precomp is not None else None
-        g_scales = out("scales", (P, 3)) if scales is not None else None
-        g_rot = out("rotations", (P, 4)) if rotations is not None else None
-        g_cov = torch.empty((P, 6), **f32) if cov3Ds_precomp is not None else None
+        if pose_only:
+            g_means = g_opac = g_sh = g_colors = g_scales = g_rot = g_cov = None
+        else:
+            g_means = out("means3D", (P, 3))
+            g_opac = out("opacities", (P, 1))
+            g_sh = out("shs", (P, M, 3)) if sh is not None else None
+            g_colors = torch.empty((P, 3), **f32) if colors_precomp is not None else None
+            g_scales = out("scales", (P, 3)) if scales is not None else None
+            g_rot = out("rotations", (P, 4)) if rotations is not None else None
+            g_cov = torch.empty((P, 6), **f32) if cov3Ds_precomp is not None else None
         scratch = st.get_scratch(P)
         if not saved.pending.done:  # a forward that did not wait for its count: it has arrived by now
             st.read(saved.pending, block=True)
         if saved.pending.overflow:
-            raise RuntimeError(f"rasterizer: this frame needed {saved.pending.num_rendered} (Gaussian, tile) instances but its "
+            raise CapacityOverflow(f"rasterizer: this frame needed {saved.pending.num_rendered} (Gaussian, tile) instances but its "
                                f"binning buffer held {saved.pending.r_cap}; it was rendered empty. The capacity has been raised: "
                                "render it again (set_capacity_checks('sync') makes every forward check its own count).")
-        camera = any(ctx.needs_input_grad[9:])  # only present when rasterize_gaussians passed the camera tensors
-        hook = _GRAD_RECORD_HOOK[0]
         if camera and hook is not None:
             raise RuntimeError("rasterizer: camera gradients (viewmatrix / projmatrix / campos with requires_grad) are not "
                                "available with a gradient-record exchange hook (set_grad_record_hook, tile-sharded frames)")
@@ -373,7 +385,11 @@ class _RasterizeGaussians(torch.autograd.Function):
                     C.c_void_p(saved.counters), _ptr(T_map), _ptr(hit_depth), _ptr(grad_out_color), _ptr(grad_out_depth), _ptr(scratch),
                     _ptr(g_means), _ptr(g_sh), _ptr(g_colors), _ptr(g_opac), _ptr(g_scales), _ptr(g_rot), _ptr(g_cov), None,
                     C.c_void_p(stream))
-            if grad_T is not None:
+            if pose_only:
+                cam_scratch = torch.empty((int(L.rtg_splat_camera_scratch_bytes(P)),), dtype=torch.uint8, device=device)
+                check(L.rtg_splat_backward_pose(*args[:19], _ptr(grad_T), _ptr(scratch), _ptr(g_cam), _ptr(cam_scratch), args[-1]),
+                      "rtg_splat_backward_pose")
+            elif grad_T is not None:
                 args_T = args[:19] + (_ptr(grad_T),) + args[19:]  # dL_dT goes right after dL_ddepth
                 if hook is None:
                     cam_out = (None, None)
@@ -466,7 +482,9 @@ def set_grad_record_hook(fn):
 
 def rasterize_gaussians(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, tile_mask, raster_settings):
     """With grad mode on and any of raster_settings.viewmatrix / projmatrix / campos requiring grad, the backward also
-    returns their gradients (dL/d of each tensor as stored, rtg_splat_backward_camera); otherwise they are constants."""
+    returns their gradients (dL/d of each tensor as stored, rtg_splat_backward_camera); otherwise they are constants. If
+    none of the seven Gaussian inputs requires grad either (a frozen map, pose refinement), the backward computes the
+    camera gradient alone (rtg_splat_backward_pose) and returns None for the Gaussians."""
     cam = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
     if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in cam):
         return _RasterizeGaussians.apply(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, tile_mask,

@@ -273,6 +273,56 @@ typedef struct RtgPoseAdam {
 } RtgPoseAdam;
 int rtg_pose_adam_step(const RtgPoseAdam *s, void *stream);
 
+/* ---- Gauss-Newton pose step (forward-mode tangents of the render) ---------------------------------------------------
+ * Pose and twist as in rtg_pose_adam_step: W2C(xi) = exp(xi^) W2C with xi = (rho, phi); under it a view-space point moves
+ * as rho + phi x p_c, a view-space direction as phi x n, the view rotation as [phi]x W and campos as -W^T rho. The
+ * tangents are those of the render the forward (the workspaces and counters of one rtg_splat_forward) produced; the
+ * discrete decisions (cull, tile and patch cut-offs, 1/255, opaque hit, plane test, T_threshold), the 1.3*tanfov clamp
+ * of the EWA Jacobian, clamped SH channels and the intrinsics are not differentiated, as in the reverse-mode gradients.
+ *
+ * rtg_splat_pose_gn_scratch_bytes: device scratch of both entry points (per-Gaussian tangent rows, per-tile partial sums;
+ * 16-byte aligned). */
+size_t rtg_splat_pose_gn_scratch_bytes(int32_t P, int32_t H, int32_t W);
+
+/* rtg_splat_pose_tangents: J (6, 4, H, W) fp32, every element written: J[k] = (dC_r, dC_g, dC_b, dD) / dxi_k of the
+ * forward's colour and depth. A pixel without a depth hit, or in a never-rendered or masked-out tile, has depth tangent 0
+ * (and, in such a tile, colour tangent 0). Gaussian inputs as in rtg_splat_backward_pose; hit_image = the forward's
+ * hit_depth. Validates on the host before any CUDA work. */
+int rtg_splat_pose_tangents(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                            const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                            const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
+                            const int32_t *hit_image, void *scratch, float *J, void *stream);
+
+/* rtg_splat_pose_gn_step: one damped Gauss-Newton step of the pose on the device. With the pixel sets of rtg_loss_l1 (S_c:
+ * the render_mask pixels, or all; S_d: hit_depth != -1, gt_depth > 0, depth - gt_depth < depth_error_max (signed), in the
+ * mask), N_c = 3 |S_c|, N_d = |S_d|, the objective is
+ *   E = 1/2 [ color_weight / N_c sum_{S_c} sum_ch (C - C^)^2 + depth_weight / N_d sum_{S_d} (D - D^)^2 ]
+ * (an empty set contributes 0). H = sum w J^T J and g = sum w J^T r are formed in double with a fixed summation order
+ * (identical inputs give bit-identical sums), damped as the ICP step, H + damping * trace(H) * I, solved xi = -H^-1 g and
+ * applied as W2C <- exp(xi^) W2C in double; viewmatrix, projmatrix and campos are rewritten in place. A singular system,
+ * N_c + N_d = 0 or an overflowed forward leaves the pose and the arrays unchanged. `report` (RTG_POSE_GN_REPORT doubles,
+ * device) receives E before the step, its colour and depth parts, N_c, N_d, |rho|, |phi| and the status. Nothing is read
+ * back to the host. Validates on the host before any CUDA work. */
+#define RTG_POSE_GN_REPORT_LEN 8
+enum { RTG_POSE_GN_OK = 0, RTG_POSE_GN_SINGULAR = 1, RTG_POSE_GN_EMPTY = 2, RTG_POSE_GN_OVERFLOW = 3 };
+typedef struct RtgPoseGN {
+    double *pose;                                       /* 16, W2C row-major, updated in place */
+    const float *projection;                            /* 16 */
+    float *viewmatrix, *projmatrix, *campos;            /* 16, 16, 3: rewritten from the pose */
+    const float *render, *depth;                        /* (3, H, W), (H, W): the forward's colour and depth */
+    const int32_t *hit_depth;                           /* (H, W): the forward's depth hit map */
+    const float *gt_color, *gt_depth;                   /* (3, H, W) or (H, W, 3) (gt_channels_last), (H, W) */
+    const uint8_t *render_mask;                         /* (H, W) or NULL */
+    void *scratch;                                      /* rtg_splat_pose_gn_scratch_bytes(P, H, W) */
+    double *report;                                     /* RTG_POSE_GN_REPORT_LEN */
+    float color_weight, depth_weight, depth_error_max, damping;
+    int32_t gt_channels_last, _pad;
+} RtgPoseGN;
+int rtg_splat_pose_gn_step(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                           const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                           const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
+                           const RtgPoseGN *s, void *stream);
+
 /* Replaces CudaRasterizer::Rasterizer::markVisible (rasterizer.h:21-26, rasterizer_impl.cu:145-157). */
 int rtg_splat_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix,
                            uint8_t *present, void *stream);

@@ -65,6 +65,18 @@ class RtgPoseAdam(C.Structure):
                 + [("step", C.c_int32)])
 
 
+class RtgPoseGN(C.Structure):
+    """include/rtg_splat_b200.h: RtgPoseGN (field order is the ABI)."""
+    _fields_ = ([(n, C.c_void_p) for n in ("pose", "projection", "viewmatrix", "projmatrix", "campos", "render", "depth", "hit_depth",
+                                           "gt_color", "gt_depth", "render_mask", "scratch", "report")]
+                + [(n, C.c_float) for n in ("color_weight", "depth_weight", "depth_error_max", "damping")]
+                + [("gt_channels_last", C.c_int32), ("_pad", C.c_int32)])
+
+
+RTG_POSE_GN_REPORT_LEN = 8
+POSE_GN_STATUS = {0: "ok", 1: "singular", 2: "empty", 3: "overflow"}
+
+
 class RtgIcpLevel(C.Structure):
     _fields_ = [("vertex0", C.c_void_p), ("normal0", C.c_void_p), ("vertex1", C.c_void_p), ("normal1", C.c_void_p),
                 ("H", C.c_int32), ("W", C.c_int32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
@@ -96,6 +108,11 @@ SIGNATURES = {
     # rtg_splat_backward_dt's arguments up to grad2d_scratch, then dL_dcamera, camera_scratch, stream
     "rtg_splat_backward_pose": (C.c_int, _BWD_ARGS[:19] + [_VP, _VP] + [_VP, _VP, _VP]),
     "rtg_pose_adam_step": (C.c_int, [C.POINTER(RtgPoseAdam), _VP]),
+    "rtg_splat_pose_gn_scratch_bytes": (C.c_size_t, [_I32, _I32, _I32]),
+    # view, P, M, 6 Gaussian inputs, 3 workspaces, R_cap, counters, then hit_image, scratch, J / the step's state, stream
+    "rtg_splat_pose_tangents": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP] + [_VP] * 4),
+    "rtg_splat_pose_gn_step": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
+                               + [C.POINTER(RtgPoseGN), _VP]),
     "rtg_splat_mark_visible": (C.c_int, [_I32, _VP, _VP, _VP, _VP, _VP]),
     "rtg_adam_step": (C.c_int, [C.POINTER(RtgAdamGroup), _I32, _F, _F, _F, _I32, _VP]),
     "rtg_map_adam_step": (C.c_int, [C.POINTER(RtgMapStep), _VP]),

@@ -127,56 +127,10 @@ __global__ void __launch_bounds__(1) pose_adam_kernel(const RtgPoseAdam s, const
         xi[k] = -(lr / bc1) * m / (sqrt(v) / bc2_sqrt + (double)s.eps);
     }
 
-    // exp(xi^) = [[R, V rho], [0, 1]], R = I + a K + b K^2, V = I + b K + c K^2, K = [phi]x
-    const double p0 = xi[3], p1 = xi[4], p2 = xi[5];
-    const double th2 = p0 * p0 + p1 * p1 + p2 * p2;
-    double a, b, c;
-    if (th2 < 1e-4) {  // Taylor series; the first omitted terms are below 1e-16
-        a = 1.0 - th2 / 6.0 * (1.0 - th2 / 20.0);
-        b = 0.5 - th2 / 24.0 * (1.0 - th2 / 30.0);
-        c = 1.0 / 6.0 - th2 / 120.0 * (1.0 - th2 / 42.0);
-    } else {
-        const double th = sqrt(th2), sn = sin(th), cs = cos(th);
-        a = sn / th;
-        b = (1.0 - cs) / th2;
-        c = (th - sn) / (th2 * th);
-    }
-    const double K[3][3] = {{0.0, -p2, p1}, {p2, 0.0, -p0}, {-p1, p0, 0.0}};
+    // W2C <- exp(xi^) W2C and the three camera arrays (common.cuh)
     double E[3][4];
-#pragma unroll
-    for (int i = 0; i < 3; i++) {
-        double Vr = 0.0;
-#pragma unroll
-        for (int j = 0; j < 3; j++) {
-            const double K2 = K[i][0] * K[0][j] + K[i][1] * K[1][j] + K[i][2] * K[2][j];
-            const double I = i == j ? 1.0 : 0.0;
-            E[i][j] = I + a * K[i][j] + b * K2;
-            Vr += (I + b * K[i][j] + c * K2) * xi[j];
-        }
-        E[i][3] = Vr;
-    }
-    double N[4][4];
-#pragma unroll
-    for (int i = 0; i < 3; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) N[i][j] = E[i][0] * T[0][j] + E[i][1] * T[1][j] + E[i][2] * T[2][j] + (j == 3 ? E[i][3] : 0.0);
-#pragma unroll
-    for (int j = 0; j < 4; j++) N[3][j] = T[3][j];
-
-#pragma unroll
-    for (int i = 0; i < 16; i++) s.pose[i] = N[i / 4][i % 4];
-#pragma unroll
-    for (int r = 0; r < 4; r++)
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-            s.viewmatrix[4 * r + q] = (float)N[q][r];
-            double pm = 0.0;
-#pragma unroll
-            for (int k = 0; k < 4; k++) pm += N[k][r] * (double)s.projection[4 * k + q];
-            s.projmatrix[4 * r + q] = (float)pm;
-        }
-#pragma unroll
-    for (int i = 0; i < 3; i++) s.campos[i] = (float)-(N[0][i] * N[0][3] + N[1][i] * N[1][3] + N[2][i] * N[2][3]);
+    se3_exp_twist(xi, E);
+    pose_left_update(E, T, s.pose, s.projection, s.viewmatrix, s.projmatrix, s.campos);
 }
 
 void launch_pose_adam_step(const RtgPoseAdam &st, cudaStream_t s) {

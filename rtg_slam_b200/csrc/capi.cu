@@ -15,6 +15,8 @@
 namespace rtg {
 int launch_adam(const RtgAdamGroup *groups, int n_groups, float beta1, float beta2, float eps, int step, cudaStream_t s);
 void launch_pose_adam_step(const RtgPoseAdam &st, cudaStream_t s);
+void launch_pose_gn_normal_eq_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                   const int32_t *counters, const RtgPoseGN &st, cudaStream_t s);
 void launch_map_adam_step(const RtgMapStep &st, cudaStream_t s);
 void launch_history_merge(const RtgHistoryMerge &m, cudaStream_t s);
 void launch_map_activate(int P, const float *scaling_raw, const float *rotation_raw, const float *opacity_raw, float *scales_out,
@@ -513,6 +515,83 @@ int rtg_splat_backward_pose(const RtgSplatView *view, int32_t P, int32_t M, cons
     rtg::launch_render_bwd(vp, g, b, img, counters, final_T, hit_image, dL_dcolor, dL_ddepth, grad2d_scratch, s, dL_dT);
     rtg::launch_preprocess_bwd_pose(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count, grad2d_scratch,
                                     dL_dcamera, camera_scratch, s);
+    return check_launch(who);
+}
+
+size_t rtg_splat_pose_gn_scratch_bytes(int32_t P, int32_t H, int32_t W) {
+    return (P < 0 || H <= 0 || W <= 0) ? 0 : rtg::pose_gn_scratch_bytes(P, H, W);
+}
+
+// Checks shared by the two tangent entry points: the forward's state and the Gaussian inputs it was rendered from.
+static int validate_pose_tangent_inputs(const char *who, const RtgSplatView *view, int32_t P, int32_t M, const float *means3D,
+                                        const float *shs, const float *colors_precomp, const float *scales, const float *rotations,
+                                        const float *cov3D_precomp, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                                        int64_t R_cap, const int32_t *counters, const int32_t *hit_image, const void *scratch) {
+    int rc = validate_view(view, who);
+    if (rc) return rc;
+    if (P < 1) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": P must be >= 1");
+    if (R_cap < 0) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": R_cap < 0");
+    if (!means3D || !geom_ws || !img_ws || !bin_ws || !counters || !hit_image || !scratch)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pointer");
+    if ((shs == nullptr) == (colors_precomp == nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "Please provide excatly one of either SHs or precomputed colors!");
+    if (((scales == nullptr || rotations == nullptr) && cov3D_precomp == nullptr) ||
+        ((scales != nullptr || rotations != nullptr) && cov3D_precomp != nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
+    if (shs && (M < (view->sh_degree + 1) * (view->sh_degree + 1) || M > 16))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": M must hold (sh_degree+1)^2 coefficients and be <= 16");
+    if ((((uintptr_t)scratch) & 15) || (((uintptr_t)rotations) & 15) || (M == 16 && (((uintptr_t)shs) & 15)))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": scratch / rotations / shs must be 16-byte aligned");
+    return RTG_OK;
+}
+
+int rtg_splat_pose_tangents(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                            const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                            const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
+                            const int32_t *hit_image, void *scratch, float *J, void *stream) {
+    const char *who = "rtg_splat_pose_tangents";
+    int rc = validate_pose_tangent_inputs(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws,
+                                          img_ws, bin_ws, R_cap, counters, hit_image, scratch);
+    if (rc) return rc;
+    if (!J) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": J is NULL");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const rtg::ViewParams vp = make_view(view);
+    const int T = vp.tiles_x * vp.tiles_y;
+    rtg::GeomState g = rtg::geom_from(const_cast<void *>(geom_ws), (size_t)P);
+    rtg::ImgState img = rtg::img_from(const_cast<void *>(img_ws), (size_t)vp.H * vp.W);
+    rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
+    rtg::launch_preprocess_tangent(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count,
+                                   reinterpret_cast<float4 *>(scratch), s);
+    rtg::launch_render_tangent_images(vp, P, g, b, img, counters, hit_image, scratch, J, s);
+    return check_launch(who);
+}
+
+int rtg_splat_pose_gn_step(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                           const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                           const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
+                           const RtgPoseGN *st, void *stream) {
+    const char *who = "rtg_splat_pose_gn_step";
+    if (!st) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": state is NULL");
+    int rc = validate_pose_tangent_inputs(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws,
+                                          img_ws, bin_ws, R_cap, counters, st->hit_depth, st->scratch);
+    if (rc) return rc;
+    if (!st->pose || !st->projection || !st->viewmatrix || !st->projmatrix || !st->campos || !st->report)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pose / projection / camera array / report");
+    if (!st->render || !st->depth || !st->gt_color || !st->gt_depth)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL render / depth / gt_color / gt_depth");
+    if ((((uintptr_t)st->pose) | ((uintptr_t)st->report)) & 7)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": pose / report must be 8-byte aligned");
+    if (!(st->damping >= 0.f) || !(st->color_weight >= 0.f) || !(st->depth_weight >= 0.f))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": damping and weights must be >= 0");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const rtg::ViewParams vp = make_view(view);
+    const int T = vp.tiles_x * vp.tiles_y;
+    rtg::GeomState g = rtg::geom_from(const_cast<void *>(geom_ws), (size_t)P);
+    rtg::ImgState img = rtg::img_from(const_cast<void *>(img_ws), (size_t)vp.H * vp.W);
+    rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
+    rtg::launch_preprocess_tangent(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count,
+                                   reinterpret_cast<float4 *>(st->scratch), s);
+    rtg::launch_pose_gn_normal_eq_step(vp, P, g, b, img, counters, *st, s);
     return check_launch(who);
 }
 

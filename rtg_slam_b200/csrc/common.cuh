@@ -20,6 +20,13 @@ namespace rtg {
 // by the per-Gaussian pass); 15: unused.
 enum { REC_COLOR = 0, REC_M0 = 3, REC_MX = 4, REC_MY = 5, REC_MXX = 6, REC_MXY = 7, REC_MYY = 8, REC_DMEAN = 9, REC_DNORMAL = 12 };
 
+// Forward-mode pose tangents (preprocess_tangent_kernel): float4 per Gaussian row, two per twist direction.
+#define RTG_TAN_ROW 12
+// Gauss-Newton terms of one residual set (colour or depth): 21 entries of J^T J (upper triangle, row by row), 6 of J^T r,
+// sum r^2, pixel count. The colour set comes first, then the depth set.
+#define RTG_GN_TERMS 29
+#define RTG_GN_ALL (2 * RTG_GN_TERMS)
+
 struct ViewParams {
     int H, W, tiles_x, tiles_y;
     float tanfovx, tanfovy, focal_x, focal_y, cx, cy;
@@ -321,6 +328,108 @@ __device__ __forceinline__ uint32_t lds32(uint32_t a) {
     uint32_t v;
     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
     return v;
+}
+
+// ------------------------------------------------------------------ 6-dof solve and SE(3) update (double)
+// Solve (JtJ + trace*damping*I) xi = -Jtr (the reference inverts the same matrix with torch.inverse on the CPU,
+// SLAM/icp.py:248-257,313-333). The damped normal matrix is symmetric positive definite: Cholesky without pivoting, fully
+// unrolled (registers only), double precision. Returns false if a pivot is not positive (degenerate view: pose unchanged).
+// Shared by the ICP iterations (icp.cu) and the render-based Gauss-Newton pose step (render.cu).
+__device__ __forceinline__ bool solve6(const double A[6][6], const double bvec[6], double x[6]) {
+    double Lm[6][6];
+    bool ok = true;
+#pragma unroll
+    for (int j = 0; j < 6; j++) {
+        double d = A[j][j];
+#pragma unroll
+        for (int k = 0; k < j; k++) d -= Lm[j][k] * Lm[j][k];
+        ok = ok && (d > 0.0);
+        const double ljj = sqrt(fmax(d, 1e-300));
+        Lm[j][j] = ljj;
+        const double inv = 1.0 / ljj;
+#pragma unroll
+        for (int i = j + 1; i < 6; i++) {
+            double v = A[i][j];
+#pragma unroll
+            for (int k = 0; k < j; k++) v -= Lm[i][k] * Lm[j][k];
+            Lm[i][j] = v * inv;
+        }
+    }
+    double y[6];
+#pragma unroll
+    for (int i = 0; i < 6; i++) {
+        double v = bvec[i];
+#pragma unroll
+        for (int k = 0; k < i; k++) v -= Lm[i][k] * y[k];
+        y[i] = v / Lm[i][i];
+    }
+#pragma unroll
+    for (int i = 5; i >= 0; i--) {
+        double v = y[i];
+#pragma unroll
+        for (int k = i + 1; k < 6; k++) v -= Lm[k][i] * x[k];
+        x[i] = v / Lm[i][i];
+    }
+    return ok;
+}
+
+// exp(xi^) of a twist xi = (rho, phi) as its top 3x4 block: [[R, V rho]], R = I + a K + b K^2, V = I + b K + c K^2,
+// K = [phi]x (closed form; Taylor series for small angles).
+__device__ __forceinline__ void se3_exp_twist(const double xi[6], double E[3][4]) {
+    const double p0 = xi[3], p1 = xi[4], p2 = xi[5];
+    const double th2 = p0 * p0 + p1 * p1 + p2 * p2;
+    double a, b, c;
+    if (th2 < 1e-4) {  // Taylor series; the first omitted terms are below 1e-16
+        a = 1.0 - th2 / 6.0 * (1.0 - th2 / 20.0);
+        b = 0.5 - th2 / 24.0 * (1.0 - th2 / 30.0);
+        c = 1.0 / 6.0 - th2 / 120.0 * (1.0 - th2 / 42.0);
+    } else {
+        const double th = sqrt(th2), sn = sin(th), cs = cos(th);
+        a = sn / th;
+        b = (1.0 - cs) / th2;
+        c = (th - sn) / (th2 * th);
+    }
+    const double K[3][3] = {{0.0, -p2, p1}, {p2, 0.0, -p0}, {-p1, p0, 0.0}};
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+        double Vr = 0.0;
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            const double K2 = K[i][0] * K[0][j] + K[i][1] * K[1][j] + K[i][2] * K[2][j];
+            const double I = i == j ? 1.0 : 0.0;
+            E[i][j] = I + a * K[i][j] + b * K2;
+            Vr += (I + b * K[i][j] + c * K2) * xi[j];
+        }
+        E[i][3] = Vr;
+    }
+}
+
+// W2C <- exp(xi^) W2C for the double pose T (row-major in `pose`), then the three arrays the rasterizer reads:
+// viewmatrix = W2C^T, projmatrix = viewmatrix @ projection, campos = -R^T t.
+__device__ __forceinline__ void pose_left_update(const double E[3][4], const double T[4][4], double *pose, const float *projection,
+                                                 float *viewmatrix, float *projmatrix, float *campos) {
+    double N[4][4];
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) N[i][j] = E[i][0] * T[0][j] + E[i][1] * T[1][j] + E[i][2] * T[2][j] + (j == 3 ? E[i][3] : 0.0);
+#pragma unroll
+    for (int j = 0; j < 4; j++) N[3][j] = T[3][j];
+
+#pragma unroll
+    for (int i = 0; i < 16; i++) pose[i] = N[i / 4][i % 4];
+#pragma unroll
+    for (int r = 0; r < 4; r++)
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+            viewmatrix[4 * r + q] = (float)N[q][r];
+            double pm = 0.0;
+#pragma unroll
+            for (int k = 0; k < 4; k++) pm += N[k][r] * (double)projection[4 * k + q];
+            projmatrix[4 * r + q] = (float)pm;
+        }
+#pragma unroll
+    for (int i = 0; i < 3; i++) campos[i] = (float)-(N[0][i] * N[0][3] + N[1][i] * N[1][3] + N[2][i] * N[2][3]);
 }
 #endif
 

@@ -186,46 +186,7 @@ __device__ __forceinline__ void se3_update(const double xi[6], float *pose) {
     // the last row of exp(xi) is (0, 0, 0, 1): the pose's last row is unchanged
 }
 
-// Solve (JtJ + trace*damping*I) xi = -Jtr (the reference inverts the same matrix with torch.inverse on the CPU,
-// SLAM/icp.py:248-257,313-333). The damped normal matrix is symmetric positive definite: Cholesky without pivoting, fully
-// unrolled (registers only), double precision. Returns false if a pivot is not positive (degenerate view: pose unchanged).
-__device__ __forceinline__ bool solve6(const double A[6][6], const double bvec[6], double x[6]) {
-    double Lm[6][6];
-    bool ok = true;
-#pragma unroll
-    for (int j = 0; j < 6; j++) {
-        double d = A[j][j];
-#pragma unroll
-        for (int k = 0; k < j; k++) d -= Lm[j][k] * Lm[j][k];
-        ok = ok && (d > 0.0);
-        const double ljj = sqrt(fmax(d, 1e-300));
-        Lm[j][j] = ljj;
-        const double inv = 1.0 / ljj;
-#pragma unroll
-        for (int i = j + 1; i < 6; i++) {
-            double v = A[i][j];
-#pragma unroll
-            for (int k = 0; k < j; k++) v -= Lm[i][k] * Lm[j][k];
-            Lm[i][j] = v * inv;
-        }
-    }
-    double y[6];
-#pragma unroll
-    for (int i = 0; i < 6; i++) {
-        double v = bvec[i];
-#pragma unroll
-        for (int k = 0; k < i; k++) v -= Lm[i][k] * y[k];
-        y[i] = v / Lm[i][i];
-    }
-#pragma unroll
-    for (int i = 5; i >= 0; i--) {
-        double v = y[i];
-#pragma unroll
-        for (int k = i + 1; k < 6; k++) v -= Lm[k][i] * x[k];
-        x[i] = v / Lm[i][i];
-    }
-    return ok;
-}
+// (solve6, the damped 6x6 Cholesky solve: common.cuh)
 
 // One Gauss-Newton iteration (compute_residuals_jacobian + compute_jtj/jtr + GN_solver, SLAM/icp.py:52-130).
 __global__ void __launch_bounds__(ICP_THREADS) icp_iter_kernel(const float *__restrict__ vertex0, const float *__restrict__ normal0,

@@ -29,6 +29,11 @@ void launch_preprocess_bwd_pose(const ViewParams &vp, int P, int M, const float 
                                 const float *shs, const float *cov3D_precomp, const GeomState &g, const uint32_t *vis_count,
                                 float *rec, float *dL_dcamera, void *camera_scratch, cudaStream_t s);
 
+// forward-mode pose tangents of the visible Gaussians (RTG_TAN_ROW float4 per row, indexed by Gaussian id)
+void launch_preprocess_tangent(const ViewParams &vp, int P, int M, const float *means, const float *scales, const float *rots,
+                               const float *shs, const float *cov3D_precomp, const GeomState &g, const uint32_t *vis_count,
+                               float4 *tan, cudaStream_t s);
+
 // binning.cu
 void launch_tile_histogram(const ViewParams &vp, int P, const GeomState &g, const int *radii, const int *tile_mask, const BinState &b,
                            cudaStream_t s);
@@ -44,6 +49,10 @@ void launch_render_fwd(const ViewParams &vp, const GeomState &g, const BinState 
 void launch_render_bwd(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img, const int32_t *counters,
                        const float *final_T, const int *hit_image, const float *dL_dcolor, const float *dL_ddepth, float *rec,
                        cudaStream_t s, const float *dL_dT = nullptr);  // dL_dT: (H, W) dL/dT_map, or NULL
+// pose Gauss-Newton: scratch = the tangent rows (read) and the per-tile partial sums
+size_t pose_gn_scratch_bytes(int P, int H, int W);
+void launch_render_tangent_images(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                  const int32_t *counters, const int *hit_image, void *scratch, float *J, cudaStream_t s);
 
 // mapstats.cu
 void launch_gs_error(int H, int W, int P, const float *color_err, const float *depth_err, const float *normal_err,

@@ -827,7 +827,116 @@ __global__ void __launch_bounds__(RTG_CAM_TERMS * 32) camera_grad_final_kernel(c
     else if (threadIdx.x < 8) dL_dcamera[16 + 4 * (threadIdx.x - 4) + 2] = 0.f;
 }
 
+// ------------------------------------------------------------------ forward-mode pose tangents
+// Tangents of one visible Gaussian's splat along the six directions of a left twist xi = (rho, phi) of the pose at zero,
+// W2C(xi) = exp(xi^) W2C: the view-space centre moves as dp_c = rho + phi x p_c, the view rotation as dW = [phi]x W and
+// the camera centre as -W^T rho. Row `idx` of `tan` (RTG_TAN_ROW float4) holds, for direction k, [2k] = (d pixel x,
+// d pixel y, d conic.x, d conic.y), [2k+1] = (d conic.z, d rgb). Not differentiated, as in the reverse-mode gradients: the
+// 1.3*tanfov clamp of the EWA Jacobian (a clamped coordinate does not move), the clamped SH channels (bwd_sh zeroes them),
+// the cull. The SH colour moves with the view direction only: d rgb_ch = (W g_ch) . rho with g_ch = d rgb_ch / d mean.
+__global__ void __launch_bounds__(256) preprocess_tangent_kernel(const ViewParams vp, const int M, const float *__restrict__ means,
+                                                                 const float *__restrict__ scales, const float *__restrict__ rots,
+                                                                 const float *__restrict__ shs, const float *__restrict__ cov3D_precomp,
+                                                                 const GeomState g, const uint32_t *__restrict__ vis_count,
+                                                                 float4 *__restrict__ tan) {
+    __shared__ float s_m[36];
+    if (threadIdx.x < 16) s_m[threadIdx.x] = vp.view[threadIdx.x];
+    else if (threadIdx.x < 32) s_m[threadIdx.x] = vp.proj[threadIdx.x - 16];
+    else if (threadIdx.x < 35) s_m[threadIdx.x] = vp.campos[threadIdx.x - 32];
+    __syncthreads();
+    const uint32_t V = *vis_count;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if ((uint32_t)i >= V) return;
+    const int idx = (int)g.vis_list[i];
+    const float *vm = s_m, *pm = s_m + 16;
+    const size_t i3 = 3 * (size_t)idx;
+    const float3 mean = make_float3(means[i3], means[i3 + 1], means[i3 + 2]);
+
+    float c6[6];
+    if (cov3D_precomp == nullptr) {
+        float R[3][3];
+        quat_to_R(reinterpret_cast<const float4 *>(rots)[idx], R);
+        cov3d_from(make_float3(scales[i3], scales[i3 + 1], scales[i3 + 2]), vp.scale_modifier, R, c6);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 6; k++) c6[k] = cov3D_precomp[6 * (size_t)idx + k];
+    }
+    const float3 pc = xform4x3(mean, vm);
+    float A0[3], A1[3], AV0[3], AV1[3], a, b, c, txtz, tytz;
+    float3 t;
+    ewa_A(pc, vm, vp.focal_x, vp.focal_y, vp.tanfovx, vp.tanfovy, A0, A1, t, txtz, tytz);
+    const float limx = 1.3f * vp.tanfovx, limy = 1.3f * vp.tanfovy;
+    const float xg = (txtz < -limx || txtz > limx) ? 0.f : 1.f;
+    const float yg = (tytz < -limy || tytz > limy) ? 0.f : 1.f;
+    cov2d_from(A0, A1, c6, AV0, AV1, a, b, c);
+    const float det_inv = 1.f / (a * c - b * b);
+    const float3 conic = make_float3(c * det_inv, -b * det_inv, a * det_inv);
+    const float4 clip = xform4x4(mean, pm);
+    const float pw = 1.0f / (clip.w + 0.0000001f);
+    const float hx = vp.focal_x, hy = vp.focal_y;
+    const float tz = 1.f / t.z, tz2 = tz * tz, tz3 = tz2 * tz;
+    const float J00 = hx * tz, J02 = -(hx * t.x) * tz2, J11 = hy * tz, J12 = -(hy * t.y) * tz2;
+
+    // colour: d rgb / d rho = W g_ch (rows of W = vm[k + 4j]); none for precomputed colours
+    float3 drgb_drho[3] = {make_float3(0.f, 0.f, 0.f), make_float3(0.f, 0.f, 0.f), make_float3(0.f, 0.f, 0.f)};
+    if (shs != nullptr) {
+        const int flags = __float_as_int(g.rgb_flags[idx].w);
+        const float3 cp = make_float3(s_m[32], s_m[33], s_m[34]);
+#pragma unroll
+        for (int ch = 0; ch < 3; ch++) {
+            const float3 gm = bwd_sh<false>(vp.sh_degree, idx, M, mean, cp, ch == 0 ? 1.f : 0.f, ch == 1 ? 1.f : 0.f,
+                                            ch == 2 ? 1.f : 0.f, flags, shs, nullptr);
+            drgb_drho[ch] = xvec4x3(gm, vm);
+        }
+    }
+
+    float4 *row = tan + (size_t)idx * RTG_TAN_ROW;
+#pragma unroll
+    for (int k = 0; k < 6; k++) {
+        // twist direction k: rho = e_k (k < 3) or phi = e_{k-3}
+        const float3 phi = make_float3(k == 3 ? 1.f : 0.f, k == 4 ? 1.f : 0.f, k == 5 ? 1.f : 0.f);
+        const float3 dp = k < 3 ? make_float3(k == 0 ? 1.f : 0.f, k == 1 ? 1.f : 0.f, k == 2 ? 1.f : 0.f)
+                                : make_float3(phi.y * pc.z - phi.z * pc.y, phi.z * pc.x - phi.x * pc.z, phi.x * pc.y - phi.y * pc.x);
+        // pixel centre: clip = (mean, 1) proj; the world point that moves p_c by dp is W^T dp
+        const float3 dw = xvec4x3T(dp, vm);
+        const float dcx = dw.x * pm[0] + dw.y * pm[4] + dw.z * pm[8], dcy = dw.x * pm[1] + dw.y * pm[5] + dw.z * pm[9];
+        const float dcw = dw.x * pm[3] + dw.y * pm[7] + dw.z * pm[11];
+        const float dpx = 0.5f * (float)vp.W * (dcx * pw - clip.x * dcw * pw * pw);
+        const float dpy = 0.5f * (float)vp.H * (dcy * pw - clip.y * dcw * pw * pw);
+        // EWA Jacobian J(t) and A = J W
+        const float dtx = xg * dp.x, dty = yg * dp.y, dtz = dp.z;
+        const float dJ00 = -hx * tz2 * dtz, dJ11 = -hy * tz2 * dtz;
+        const float dJ02 = -hx * tz2 * dtx + 2.f * hx * t.x * tz3 * dtz, dJ12 = -hy * tz2 * dty + 2.f * hy * t.y * tz3 * dtz;
+        float da = 0.f, db = 0.f, dc = 0.f;
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            const float3 col = make_float3(vm[4 * j], vm[4 * j + 1], vm[4 * j + 2]);  // column j of W
+            const float3 dcol = make_float3(phi.y * col.z - phi.z * col.y, phi.z * col.x - phi.x * col.z, phi.x * col.y - phi.y * col.x);
+            const float dA0 = dJ00 * col.x + dJ02 * col.z + J00 * dcol.x + J02 * dcol.z;
+            const float dA1 = dJ11 * col.y + dJ12 * col.z + J11 * dcol.y + J12 * dcol.z;
+            da += 2.f * dA0 * AV0[j];
+            db += dA0 * AV1[j] + dA1 * AV0[j];
+            dc += 2.f * dA1 * AV1[j];
+        }
+        // conic = (c, -b, a) / (a c - b^2)
+        const float ddet = da * c + a * dc - 2.f * b * db;
+        const float dk0 = (dc - conic.x * ddet) * det_inv, dk1 = (-db - conic.y * ddet) * det_inv, dk2 = (da - conic.z * ddet) * det_inv;
+        const float dr = k < 3 ? (k == 0 ? drgb_drho[0].x : (k == 1 ? drgb_drho[0].y : drgb_drho[0].z)) : 0.f;
+        const float dg = k < 3 ? (k == 0 ? drgb_drho[1].x : (k == 1 ? drgb_drho[1].y : drgb_drho[1].z)) : 0.f;
+        const float dbl = k < 3 ? (k == 0 ? drgb_drho[2].x : (k == 1 ? drgb_drho[2].y : drgb_drho[2].z)) : 0.f;
+        row[2 * k] = make_float4(dpx, dpy, dk0, dk1);
+        row[2 * k + 1] = make_float4(dk2, dr, dg, dbl);
+    }
+}
+
 // ------------------------------------------------------------------ launchers
+void launch_preprocess_tangent(const ViewParams &vp, int P, int M, const float *means, const float *scales, const float *rots,
+                               const float *shs, const float *cov3D_precomp, const GeomState &g, const uint32_t *vis_count,
+                               float4 *tan, cudaStream_t s) {
+    if (P <= 0) return;
+    preprocess_tangent_kernel<<<(P + 255) / 256, 256, 0, s>>>(vp, M, means, scales, rots, shs, cov3D_precomp, g, vis_count, tan);
+}
+
 void launch_preprocess_fwd(const ViewParams &vp, int P, int M, const float *means, const float *scales, const float *rots,
                            const float *opac, const float *shs, const float *colors_precomp, const float *cov3D_precomp,
                            const int *tile_mask, const GeomState &g, int *radii, uint32_t *tile_count, uint32_t *tile_touched,

@@ -27,6 +27,7 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "prof.h"
+#include "../../include/rtg_splat_b200.h"
 
 namespace rtg {
 
@@ -747,6 +748,272 @@ __global__ void BWD_BOUNDS render_bwd_kernel(const ViewParams vp, const GeomStat
 
     depth_hit_grad(vp, g, hit_image, dL_ddepth, rec, px, pyA, pidA, insA);
     depth_hit_grad(vp, g, hit_image, dL_ddepth, rec, px, pyB, pidB, insB);
+}
+
+// ------------------------------------------------------------------ forward-mode pose tangents
+// Tangent images of the forward's render along the six twist directions (preprocess_tangent_kernel holds the per-Gaussian
+// tangents). One CTA per tile, in the forward's launch order, one pixel per thread on the forward's 8x4 warp patches. The
+// tile's list is replayed front to back up to the longest prefix its pixels blended (max n_contrib), with the forward's
+// decisions: the same patch masks, the same alpha function (pair_alpha: the exact expression inside the band around 1/255)
+// and a pixel's own n_contrib. Per pixel: T, its 6 tangents and the 18 colour tangents of
+//   C = sum c_i alpha_i T_i + T_final bg,   d alpha_i = au_i d power_i   (0 where alpha is clamped at 0.99),
+// and the depth tangent of the hit Gaussian (hit_image), on the forward's plane / centre branch. No parameter array is read.
+//   TAN_IMAGES:    J (6, 4, H, W): colour channels then depth, per direction; zeros where the tile is not rendered.
+//   TAN_NORMAL_EQ: the residuals against the frame and the pixel selection of rtg_loss_l1, summed per tile into the
+//                  RTG_GN_ALL Gauss-Newton terms (warp butterfly in double, warps in order, one row per TILE ID so that
+//                  the launch order, which varies between runs, does not change any sum). No atomics.
+enum { TAN_IMAGES = 0, TAN_NORMAL_EQ = 1 };
+struct GnInputs {
+    const float *render, *depth, *gt_color, *gt_depth;
+    const uint8_t *mask;
+    int channels_last;
+    float depth_error_max;
+    double *partial;  // [tiles][RTG_GN_ALL]
+};
+
+template <int MODE>
+__global__ void __launch_bounds__(256) render_tangent_kernel(const ViewParams vp, const GeomState g, const BinState b, const ImgState img,
+                                                             const int *__restrict__ counters, const int *__restrict__ hit_image,
+                                                             const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs in) {
+    __shared__ float4 s_s0[BATCH], s_s1[BATCH], s_rgb[BATCH];
+    __shared__ int s_id[BATCH];
+    __shared__ uint32_t s_mask[BATCH];
+    __shared__ uint32_t s_max[8];
+    __shared__ double s_red[MODE == TAN_NORMAL_EQ ? 8 : 1][RTG_GN_ALL];
+
+    const int tile = (int)b.active[blockIdx.x];
+    int px, py;
+    bool inside;
+    pixel_of(vp, tile, px, py, inside);
+    const int pix = vp.W * py + px;
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int n = counters[2] != 0 ? 0 : (int)b.tile_count[(size_t)tile * RTG_CNT_STRIDE];
+    const uint32_t start = b.tile_offset[tile];
+    const uint32_t last = (inside && n > 0) ? img.n_contrib[pix] : 0u;
+    uint32_t wmax = last;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(FULL, wmax, o));
+    if (lane == 0) s_max[w] = wmax;
+    __syncthreads();
+    uint32_t m = 0;
+#pragma unroll
+    for (int k = 0; k < 8; k++) m = max(m, s_max[k]);
+
+    const float pxf = (float)px, pyf = (float)py;
+    const float tx0 = (float)((tile % vp.tiles_x) * RTG_TILE), ty0 = (float)((tile / vp.tiles_x) * RTG_TILE);
+    float T = 1.f, dT[6], dC[3][6];
+#pragma unroll
+    for (int k = 0; k < 6; k++) { dT[k] = 0.f; dC[0][k] = dC[1][k] = dC[2][k] = 0.f; }
+
+    const int rounds = ((int)m + BATCH - 1) / BATCH;
+    for (int i = 0; i < rounds; i++) {
+        __syncthreads();  // the previous round has been consumed
+        if (i * BATCH + (int)threadIdx.x < (int)m) {
+            const int id = (int)b.point_list[start + (size_t)i * BATCH + threadIdx.x];
+            const float4 s0 = __ldg(g.splat + 2 * (size_t)id), s1 = __ldg(g.splat + 2 * (size_t)id + 1);
+            s_id[threadIdx.x] = id;
+            s_s0[threadIdx.x] = s0;
+            s_s1[threadIdx.x] = s1;
+            s_rgb[threadIdx.x] = __ldg(g.rgb_flags + id);
+            s_mask[threadIdx.x] = patch_mask(s0, s1, tx0, ty0);
+        }
+        __syncthreads();
+        const int cnt = min(BATCH, (int)m - i * BATCH);
+        for (int c = 0; c < ((cnt + 31) >> 5); c++) {
+            const int e = (c << 5) + lane;
+            const uint32_t mm = e < cnt ? s_mask[e] : 0u;
+            uint32_t bits = __ballot_sync(FULL, (mm >> w) & 1u);
+            while (bits) {
+                const int j = (c << 5) + __ffs(bits) - 1;
+                bits &= bits - 1;
+                const uint32_t pos = (uint32_t)(i * BATCH + j);
+                const float4 s0 = s_s0[j], s1 = s_s1[j];
+                const float dx = s0.x - pxf, dy = s0.y - pyf;
+                const float power = pair_power(s1.x, s1.y, s1.z, dx, dy);
+                float alpha, au;
+                // the backward's decisions: its own prefix, the same pretest, the same alpha function
+                const bool ok = pos < last && RTG_FWD_PRETEST(power, s0.z) && pair_alpha(power, s1.w, s0.w, alpha, au);
+                if (!__any_sync(FULL, ok)) continue;
+                if (ok) {
+                    const float4 *tr = tan + (size_t)s_id[j] * RTG_TAN_ROW;
+                    const float4 col = s_rgb[j];
+                    const float dadp = au <= 0.99f ? au : 0.f;  // d alpha / d power
+                    const float gx = -(s1.x * dx + s1.y * dy), gy = -(s1.z * dy + s1.y * dx);  // d power / d centre
+                    const float wgt = alpha * T;
+#pragma unroll
+                    for (int k = 0; k < 6; k++) {
+                        const float4 ta = __ldg(tr + 2 * k), tb = __ldg(tr + 2 * k + 1);
+                        const float dpow = gx * ta.x + gy * ta.y - 0.5f * dx * dx * ta.z - dx * dy * ta.w - 0.5f * dy * dy * tb.x;
+                        const float dal = dadp * dpow;
+                        const float dw = dal * T + alpha * dT[k];  // d (alpha T)
+                        dC[0][k] += tb.y * wgt + col.x * dw;
+                        dC[1][k] += tb.z * wgt + col.y * dw;
+                        dC[2][k] += tb.w * wgt + col.z * dw;
+                        dT[k] = dT[k] * (1.f - alpha) - T * dal;
+                    }
+                    T = T * (1.f - alpha);
+                }
+            }
+        }
+    }
+
+    // colour: the background term T_final bg; depth: the hit Gaussian's plane or centre depth
+    const float bg0 = __ldg(vp.bg), bg1 = __ldg(vp.bg + 1), bg2 = __ldg(vp.bg + 2);
+#pragma unroll
+    for (int k = 0; k < 6; k++) { dC[0][k] += bg0 * dT[k]; dC[1][k] += bg1 * dT[k]; dC[2][k] += bg2 * dT[k]; }
+    float dD[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    const int gid = (inside && n > 0) ? hit_image[pix] : -1;  // a never-rendered tile's hit map holds 0, not a hit
+    if (gid >= 0) {
+        const float3 ray = pixel_ray(px, py, vp.focal_x, vp.focal_y, vp.cx, vp.cy);
+        const float4 h0 = __ldg(g.hit + 2 * (size_t)gid), h1 = __ldg(g.hit + 2 * (size_t)gid + 1);
+        const float3 nc = make_float3(h0.x, h0.y, h0.z), pc = make_float3(h1.x, h1.y, h1.z);
+        const float num = pc.x * nc.x + pc.y * nc.y + pc.z * nc.z;
+        const float ndotr = nc.x * ray.x + nc.y * ray.y + nc.z * ray.z;
+        const float tt = (float)((double)num / ((double)ndotr + 1e-8));
+        // surfel_depth's decision
+        if (fabsf(tt * ray.z - pc.z) <= h0.w * vp.depth_thr && fabsf(ndotr) >= vp.normal_thr) {
+            // D = ray.z (n.p_c) / (n.ray + 1e-8): d(n.p_c) = n.rho (the rotation moves n and p_c alike), d(n.ray) = phi.(n x ray)
+            const float inv_nr = 1.f / (float)((double)ndotr + 1e-8);
+            const float s = -ray.z * num * inv_nr * inv_nr;
+            dD[0] = ray.z * nc.x * inv_nr; dD[1] = ray.z * nc.y * inv_nr; dD[2] = ray.z * nc.z * inv_nr;
+            dD[3] = s * (nc.y * ray.z - nc.z * ray.y); dD[4] = s * (nc.z * ray.x - nc.x * ray.z); dD[5] = s * (nc.x * ray.y - nc.y * ray.x);
+        } else {  // centre depth: (rho + phi x p_c).z
+            dD[2] = 1.f; dD[3] = pc.y; dD[4] = -pc.x;
+        }
+    }
+
+    if constexpr (MODE == TAN_IMAGES) {
+        if (inside) {
+            const size_t HW = (size_t)vp.H * vp.W;
+#pragma unroll
+            for (int k = 0; k < 6; k++) {
+                float *o = J + (size_t)(4 * k) * HW + pix;
+                o[0] = dC[0][k]; o[HW] = dC[1][k]; o[2 * HW] = dC[2][k]; o[3 * HW] = dD[k];
+            }
+        }
+    } else {
+        const int N = vp.H * vp.W;
+        float rc[3] = {0.f, 0.f, 0.f}, rd = 0.f;
+        bool sc = inside && (in.mask == nullptr || in.mask[pix] != 0), sd = false;
+        if (sc) {
+#pragma unroll
+            for (int ch = 0; ch < 3; ch++) {
+                const float gt = in.channels_last ? in.gt_color[3 * (size_t)pix + ch] : in.gt_color[(size_t)ch * N + pix];
+                rc[ch] = in.render[(size_t)ch * N + pix] - gt;
+            }
+            const float gd = in.gt_depth[pix];
+            rd = in.depth[pix] - gd;
+            sd = hit_image[pix] != -1 && gd > 0.f && rd < in.depth_error_max;  // rtg_loss_l1's depth pixels (signed error)
+        }
+        float v[RTG_GN_ALL];
+        int q = 0;
+#pragma unroll
+        for (int a = 0; a < 6; a++)
+#pragma unroll
+            for (int c = a; c < 6; c++, q++) {
+                v[q] = sc ? dC[0][a] * dC[0][c] + dC[1][a] * dC[1][c] + dC[2][a] * dC[2][c] : 0.f;
+                v[RTG_GN_TERMS + q] = sd ? dD[a] * dD[c] : 0.f;
+            }
+#pragma unroll
+        for (int a = 0; a < 6; a++) {
+            v[21 + a] = sc ? dC[0][a] * rc[0] + dC[1][a] * rc[1] + dC[2][a] * rc[2] : 0.f;
+            v[RTG_GN_TERMS + 21 + a] = sd ? dD[a] * rd : 0.f;
+        }
+        v[27] = sc ? rc[0] * rc[0] + rc[1] * rc[1] + rc[2] * rc[2] : 0.f;
+        v[28] = sc ? 1.f : 0.f;
+        v[RTG_GN_TERMS + 27] = sd ? rd * rd : 0.f;
+        v[RTG_GN_TERMS + 28] = sd ? 1.f : 0.f;
+#pragma unroll
+        for (int t = 0; t < RTG_GN_ALL; t++) {
+            double x = (double)v[t];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(FULL, x, o);
+            if (lane == 0) s_red[w][t] = x;
+        }
+        __syncthreads();
+        if (threadIdx.x < RTG_GN_ALL) {
+            double acc = 0.0;
+#pragma unroll
+            for (int k = 0; k < 8; k++) acc += s_red[k][threadIdx.x];
+            in.partial[(size_t)tile * RTG_GN_ALL + threadIdx.x] = acc;
+        }
+    }
+}
+
+// One block: the fixed-order sum of the tiles' rows (one warp per term, fixed lane stride, fixed butterfly), then on one
+// thread the weights and counts, the trace damping, solve6, exp(xi^) W2C and the three camera arrays. A singular system,
+// an empty selection or an overflowed forward leaves the pose and the arrays unchanged and sets the status.
+__global__ void __launch_bounds__(256) pose_gn_step_kernel(const int tiles, const double *__restrict__ partial,
+                                                            const int *__restrict__ counters, const RtgPoseGN s) {
+    __shared__ double s_tot[RTG_GN_ALL];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int term = w; term < RTG_GN_ALL; term += 8) {
+        double acc = 0.0;
+        for (int t = lane; t < tiles; t += 32) acc += partial[(size_t)t * RTG_GN_ALL + term];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL, acc, o);
+        if (lane == 0) s_tot[term] = acc;
+    }
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    const double *cs = s_tot, *ds = s_tot + RTG_GN_TERMS;
+    const double nc = 3.0 * cs[28], nd = ds[28];
+    const double wc = nc > 0.0 ? (double)s.color_weight / nc : 0.0, wd = nd > 0.0 ? (double)s.depth_weight / nd : 0.0;
+    double A[6][6], bvec[6], xi[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    int q = 0;
+#pragma unroll
+    for (int a = 0; a < 6; a++)
+#pragma unroll
+        for (int c = a; c < 6; c++, q++) { const double v = wc * cs[q] + wd * ds[q]; A[a][c] = v; A[c][a] = v; }
+    double trace = 0.0;
+#pragma unroll
+    for (int a = 0; a < 6; a++) trace += A[a][a];
+#pragma unroll
+    for (int a = 0; a < 6; a++) { A[a][a] += trace * (double)s.damping; bvec[a] = -(wc * cs[21 + a] + wd * ds[21 + a]); }
+    int status = RTG_POSE_GN_OK;
+    if (counters[2] != 0) status = RTG_POSE_GN_OVERFLOW;
+    else if (nc + nd == 0.0) status = RTG_POSE_GN_EMPTY;
+    else if (!solve6(A, bvec, xi)) status = RTG_POSE_GN_SINGULAR;
+    if (status == RTG_POSE_GN_OK) {
+        double Tm[4][4], E[3][4];
+#pragma unroll
+        for (int i = 0; i < 16; i++) Tm[i / 4][i % 4] = s.pose[i];
+        se3_exp_twist(xi, E);
+        pose_left_update(E, Tm, s.pose, s.projection, s.viewmatrix, s.projmatrix, s.campos);
+    } else {
+#pragma unroll
+        for (int a = 0; a < 6; a++) xi[a] = 0.0;
+    }
+    const double ec = 0.5 * wc * cs[27], ed = 0.5 * wd * ds[27];
+    double *r = s.report;
+    r[0] = ec + ed; r[1] = ec; r[2] = ed; r[3] = nc; r[4] = nd;
+    r[5] = sqrt(xi[0] * xi[0] + xi[1] * xi[1] + xi[2] * xi[2]);
+    r[6] = sqrt(xi[3] * xi[3] + xi[4] * xi[4] + xi[5] * xi[5]);
+    r[7] = (double)status;
+}
+
+size_t pose_gn_scratch_bytes(int P, int H, int W) {
+    const size_t tiles = (size_t)((W + RTG_TILE - 1) / RTG_TILE) * ((H + RTG_TILE - 1) / RTG_TILE);
+    return align_up((size_t)(P > 0 ? P : 0) * RTG_TAN_ROW * sizeof(float4), 256) + tiles * RTG_GN_ALL * sizeof(double);
+}
+static inline float4 *tan_rows(void *scratch) { return reinterpret_cast<float4 *>(scratch); }
+static inline double *gn_partial(void *scratch, int P) {
+    return reinterpret_cast<double *>(reinterpret_cast<char *>(scratch) + align_up((size_t)P * RTG_TAN_ROW * sizeof(float4), 256));
+}
+
+void launch_render_tangent_images(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                  const int32_t *counters, const int *hit_image, void *scratch, float *J, cudaStream_t s) {
+    const int T = vp.tiles_x * vp.tiles_y;
+    render_tangent_kernel<TAN_IMAGES><<<T, 256, 0, s>>>(vp, g, b, img, counters, hit_image, tan_rows(scratch), J, GnInputs{});
+}
+
+void launch_pose_gn_normal_eq_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                   const int32_t *counters, const RtgPoseGN &st, cudaStream_t s) {
+    const int T = vp.tiles_x * vp.tiles_y;
+    GnInputs in{st.render, st.depth, st.gt_color, st.gt_depth, st.render_mask, st.gt_channels_last, st.depth_error_max,
+                gn_partial(st.scratch, P)};
+    render_tangent_kernel<TAN_NORMAL_EQ><<<T, 256, 0, s>>>(vp, g, b, img, counters, st.hit_depth, tan_rows(st.scratch), nullptr, in);
+    pose_gn_step_kernel<<<1, 256, 0, s>>>(T, in.partial, counters, st);
 }
 
 void launch_render_fwd(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img, const int32_t *counters,

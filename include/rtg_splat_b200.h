@@ -323,6 +323,26 @@ int rtg_splat_pose_gn_step(const RtgSplatView *view, int32_t P, int32_t M, const
                            const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
                            const RtgPoseGN *s, void *stream);
 
+/* rtg_splat_pose_gn_step_robust: rtg_splat_pose_gn_step with a robust loss on each residual r (a colour channel, or the
+ * depth). With rho(r) = r^2 / 2 for |r| <= delta and delta |r| - delta^2 / 2 otherwise (Huber), the objective is
+ *   E = color_weight / N_c sum_{S_c} sum_ch rho_cd(C - C^) + depth_weight / N_d sum_{S_d} rho_dd(D - D^)
+ * over the same pixel sets and counts. It is minimised by iteratively reweighted least squares: each residual gets the
+ * weight w = 1 (|r| <= delta) or delta / |r|, computed in float from the float residual, H = sum w J^T J and g = sum w J^T r
+ * (g is the gradient of E); the damping, the solve, the update, the camera arrays and the report are those of
+ * rtg_splat_pose_gn_step, with the report's E, E_colour and E_depth the robust ones. RTG_ROBUST_NONE launches exactly what
+ * rtg_splat_pose_gn_step launches. Rejects a NULL `robust`, an unknown kernel and, for RTG_ROBUST_HUBER, a delta that is
+ * not positive and finite, on the host before any CUDA work (and validates the rest as rtg_splat_pose_gn_step). */
+enum { RTG_ROBUST_NONE = 0, RTG_ROBUST_HUBER = 1 };
+typedef struct RtgPoseRobust {
+    int32_t kernel;                                     /* RTG_ROBUST_NONE or RTG_ROBUST_HUBER */
+    float color_delta, depth_delta;                     /* Huber thresholds: colour units, map units */
+    int32_t _pad;
+} RtgPoseRobust;
+int rtg_splat_pose_gn_step_robust(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                                  const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                  const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
+                                  const RtgPoseGN *s, const RtgPoseRobust *robust, void *stream);
+
 /* Replaces CudaRasterizer::Rasterizer::markVisible (rasterizer.h:21-26, rasterizer_impl.cu:145-157). */
 int rtg_splat_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix,
                            uint8_t *present, void *stream);
@@ -519,6 +539,19 @@ int rtg_frame_preprocess(const float *depth_in, int32_t H, int32_t W, int32_t de
                          float sigma_space, float min_depth, float max_depth, float fx, float fy, float cx, float cy,
                          float invalid_confidence_thresh, float *depth_out, float *vertex_out, float *normal_out,
                          float *confidence_out, uint8_t *invalid_mask_out, void *ws, void *stream);
+
+/* rtg_frame_downsample: level `scale` (>= 2) of a measured frame for coarse-to-fine tracking, in one launch. Coarse pixel
+ * (i, j) covers the fine block [s i, s i + s) x [s j, s j + s); the coarse size is Hs = H / s, Ws = W / s (integer division:
+ * a trailing partial row or column is dropped). color (3, H, W) or (H, W, 3) (color_channels_last) -> color_out (3, Hs, Ws):
+ * the block mean per channel. depth (H, W) -> depth_out (Hs, Ws): the block mean when all s^2 depths are > 0, else 0.
+ * render_mask (H, W) uint8, optional -> mask_out (Hs, Ws): 1 when all s^2 pixels are nonzero, else 0. tile_mask, optional, in
+ * the rasterizer's layout (ceil(H/16), ceil(W/16)) int32 -> tile_mask_out (ceil(Hs/16), ceil(Ws/16)): 1 when any fine tile
+ * of [s tx, s tx + s) x [s ty, s ty + s), clipped to the fine grid, is nonzero. The camera of the coarse level is the
+ * caller's (tracking.level_camera). Validates on the host before any CUDA work: sizes, scale, NULL pointers, and that
+ * mask_out / tile_mask_out are given exactly when render_mask / tile_mask are. */
+int rtg_frame_downsample(const float *color, const float *depth, const uint8_t *render_mask, const int32_t *tile_mask, int32_t H,
+                         int32_t W, int32_t scale, int32_t color_channels_last, float *color_out, float *depth_out,
+                         uint8_t *mask_out, int32_t *tile_mask_out, void *stream);
 
 /* ---- per-frame consumers of the rasterizer's index / transmittance maps (SURVEY.md section 8(f) #2) ---------
  * accumulate_gaussian_error of submodules/cuda_utils (cuda_utils.cu:17-60, map_process.cu:33-245), called by

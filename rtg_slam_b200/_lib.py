@@ -77,6 +77,14 @@ RTG_POSE_GN_REPORT_LEN = 8
 POSE_GN_STATUS = {0: "ok", 1: "singular", 2: "empty", 3: "overflow"}
 
 
+class RtgPoseRobust(C.Structure):
+    """include/rtg_splat_b200.h: RtgPoseRobust (field order is the ABI)."""
+    _fields_ = [("kernel", C.c_int32), ("color_delta", C.c_float), ("depth_delta", C.c_float), ("_pad", C.c_int32)]
+
+
+RTG_ROBUST_NONE, RTG_ROBUST_HUBER = 0, 1
+
+
 class RtgIcpLevel(C.Structure):
     _fields_ = [("vertex0", C.c_void_p), ("normal0", C.c_void_p), ("vertex1", C.c_void_p), ("normal1", C.c_void_p),
                 ("H", C.c_int32), ("W", C.c_int32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
@@ -113,6 +121,8 @@ SIGNATURES = {
     "rtg_splat_pose_tangents": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP] + [_VP] * 4),
     "rtg_splat_pose_gn_step": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
                                + [C.POINTER(RtgPoseGN), _VP]),
+    "rtg_splat_pose_gn_step_robust": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
+                                      + [C.POINTER(RtgPoseGN), C.POINTER(RtgPoseRobust), _VP]),
     "rtg_splat_mark_visible": (C.c_int, [_I32, _VP, _VP, _VP, _VP, _VP]),
     "rtg_adam_step": (C.c_int, [C.POINTER(RtgAdamGroup), _I32, _F, _F, _F, _I32, _VP]),
     "rtg_map_adam_step": (C.c_int, [C.POINTER(RtgMapStep), _VP]),
@@ -132,6 +142,8 @@ SIGNATURES = {
     "rtg_ssim_loss": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _VP, _VP, _VP, _VP]),
     "rtg_normal_map": (C.c_int, [_VP, _VP, _I32, _I32, _VP, _VP]),
     "rtg_frame_preprocess": (C.c_int, [_VP, _I32, _I32, _I32, _I32] + [_F] * 9 + [_VP] * 7),
+    # color, depth, render_mask, tile_mask, H, W, scale, color_channels_last, 4 outputs, stream
+    "rtg_frame_downsample": (C.c_int, [_VP] * 4 + [_I32] * 4 + [_VP] * 4 + [_VP]),
     "rtg_accumulate_gaussian_error": (C.c_int, [_I32, _I32, _I32] + [_VP] * 5 + [_F, _F, _F, _I32] + [_VP] * 6),
     "rtg_tile_mean": (C.c_int, [_I32, _I32, _VP, _F, _VP, _VP, _VP]),
     "rtg_transmission_tile_mask": (C.c_int, [_I32, _I32, _VP, _F, _VP, _VP, _VP]),

@@ -16,7 +16,10 @@ namespace rtg {
 int launch_adam(const RtgAdamGroup *groups, int n_groups, float beta1, float beta2, float eps, int step, cudaStream_t s);
 void launch_pose_adam_step(const RtgPoseAdam &st, cudaStream_t s);
 void launch_pose_gn_normal_eq_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
-                                   const int32_t *counters, const RtgPoseGN &st, cudaStream_t s);
+                                   const int32_t *counters, const RtgPoseGN &st, const RtgPoseRobust &robust, cudaStream_t s);
+void launch_frame_downsample(const float *color, const float *depth, const uint8_t *render_mask, const int32_t *tile_mask, int H,
+                             int W, int scale, int channels_last, float *color_out, float *depth_out, uint8_t *mask_out,
+                             int32_t *tile_mask_out, cudaStream_t s);
 void launch_map_adam_step(const RtgMapStep &st, cudaStream_t s);
 void launch_history_merge(const RtgHistoryMerge &m, cudaStream_t s);
 void launch_map_activate(int P, const float *scaling_raw, const float *rotation_raw, const float *opacity_raw, float *scales_out,
@@ -566,12 +569,11 @@ int rtg_splat_pose_tangents(const RtgSplatView *view, int32_t P, int32_t M, cons
     return check_launch(who);
 }
 
-int rtg_splat_pose_gn_step(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
-                           const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
-                           const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
-                           const RtgPoseGN *st, void *stream) {
-    const char *who = "rtg_splat_pose_gn_step";
-    if (!st) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": state is NULL");
+// The step of both Gauss-Newton entry points: `robust` selects the normal-equation rows (RTG_ROBUST_NONE: the plain ones).
+static int pose_gn_step(const char *who, const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                        const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                        const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
+                        const RtgPoseGN *st, const RtgPoseRobust &robust, void *stream) {
     int rc = validate_pose_tangent_inputs(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws,
                                           img_ws, bin_ws, R_cap, counters, st->hit_depth, st->scratch);
     if (rc) return rc;
@@ -591,8 +593,36 @@ int rtg_splat_pose_gn_step(const RtgSplatView *view, int32_t P, int32_t M, const
     rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
     rtg::launch_preprocess_tangent(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count,
                                    reinterpret_cast<float4 *>(st->scratch), s);
-    rtg::launch_pose_gn_normal_eq_step(vp, P, g, b, img, counters, *st, s);
+    rtg::launch_pose_gn_normal_eq_step(vp, P, g, b, img, counters, *st, robust, s);
     return check_launch(who);
+}
+
+int rtg_splat_pose_gn_step(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                           const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                           const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
+                           const RtgPoseGN *st, void *stream) {
+    const char *who = "rtg_splat_pose_gn_step";
+    if (!st) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": state is NULL");
+    const RtgPoseRobust none{RTG_ROBUST_NONE, 0.f, 0.f, 0};
+    return pose_gn_step(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws, img_ws, bin_ws,
+                        R_cap, counters, st, none, stream);
+}
+
+int rtg_splat_pose_gn_step_robust(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                                  const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                  const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
+                                  const RtgPoseGN *st, const RtgPoseRobust *robust, void *stream) {
+    const char *who = "rtg_splat_pose_gn_step_robust";
+    if (!st) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": state is NULL");
+    if (!robust) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": robust is NULL");
+    if (robust->kernel != RTG_ROBUST_NONE && robust->kernel != RTG_ROBUST_HUBER)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": unknown robust kernel");
+    if (robust->kernel == RTG_ROBUST_HUBER &&
+        !(std::isfinite(robust->color_delta) && robust->color_delta > 0.f && std::isfinite(robust->depth_delta) &&
+          robust->depth_delta > 0.f))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": color_delta and depth_delta must be positive and finite");
+    return pose_gn_step(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws, img_ws, bin_ws,
+                        R_cap, counters, st, *robust, stream);
 }
 
 int rtg_pose_adam_step(const RtgPoseAdam *st, void *stream) {
@@ -827,6 +857,25 @@ int rtg_frame_preprocess(const float *depth_in, int32_t H, int32_t W, int32_t de
                                  invalid_confidence_thresh, depth_out, vertex_out, normal_out, confidence_out, invalid_mask_out, ws,
                                  reinterpret_cast<cudaStream_t>(stream));
     return check_launch("rtg_frame_preprocess");
+}
+
+int rtg_frame_downsample(const float *color, const float *depth, const uint8_t *render_mask, const int32_t *tile_mask, int32_t H,
+                         int32_t W, int32_t scale, int32_t color_channels_last, float *color_out, float *depth_out,
+                         uint8_t *mask_out, int32_t *tile_mask_out, void *stream) {
+    const char *who = "rtg_frame_downsample";
+    if (scale < 2) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": scale must be >= 2");
+    if (H <= 0 || W <= 0 || H / scale < 1 || W / scale < 1)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": H and W must be >= scale");
+    if (color_channels_last != 0 && color_channels_last != 1)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": color_channels_last must be 0 or 1");
+    if (!color || !depth || !color_out || !depth_out) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pointer");
+    if ((render_mask == nullptr) != (mask_out == nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": mask_out must be given exactly when render_mask is");
+    if ((tile_mask == nullptr) != (tile_mask_out == nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": tile_mask_out must be given exactly when tile_mask is");
+    rtg::launch_frame_downsample(color, depth, render_mask, tile_mask, H, W, scale, color_channels_last, color_out, depth_out,
+                                 mask_out, tile_mask_out, reinterpret_cast<cudaStream_t>(stream));
+    return check_launch(who);
 }
 
 int rtg_accumulate_gaussian_error(int32_t H, int32_t W, int32_t P, const float *screen_color_error, const float *screen_depth_error,

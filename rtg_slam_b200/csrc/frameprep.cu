@@ -70,6 +70,67 @@ __global__ void __launch_bounds__(256) confidence_mask_kernel(const int H, const
     if (invalid) invalid[idx] = bad ? 1 : 0;
 }
 
+// Level `scale` of a measured frame for coarse-to-fine tracking: coarse pixel (i, j) pools the fine block
+// [s i, s i + s) x [s j, s j + s) (a trailing partial row / column is dropped). Colour: the block mean per channel; depth:
+// the block mean when every depth is > 0, else 0; render mask: set when every pixel is set. Sums run over the block in row
+// order. One thread per coarse pixel; there are never more coarse tiles than coarse pixels, so the first threads also pool
+// one tile each: coarse tile (tx, ty) is set when any fine tile of [s tx, s tx + s) x [s ty, s ty + s) (clipped to the fine
+// grid) is set -- a coarse 16x16 tile covers exactly those s x s fine tiles.
+__global__ void __launch_bounds__(256) frame_downsample_kernel(const float *__restrict__ color, const float *__restrict__ depth,
+                                                               const uint8_t *__restrict__ render_mask,
+                                                               const int32_t *__restrict__ tile_mask, const int H, const int W,
+                                                               const int s, const int channels_last, float *__restrict__ color_out,
+                                                               float *__restrict__ depth_out, uint8_t *__restrict__ mask_out,
+                                                               int32_t *__restrict__ tile_mask_out) {
+    const int Hs = H / s, Ws = W / s;
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= Hs * Ws) return;
+    const int i = idx % Ws, j = idx / Ws;
+    const float n_block = (float)(s * s);
+    float c0 = 0.f, c1 = 0.f, c2 = 0.f, d = 0.f;
+    bool all_depth = true, all_mask = true;
+    for (int dy = 0; dy < s; dy++) {
+        const size_t row = (size_t)(s * j + dy) * W + (size_t)s * i;
+        for (int dx = 0; dx < s; dx++) {
+            const size_t p = row + dx;
+            if (channels_last) {
+                c0 += color[3 * p]; c1 += color[3 * p + 1]; c2 += color[3 * p + 2];
+            } else {
+                c0 += color[p]; c1 += color[(size_t)H * W + p]; c2 += color[2 * (size_t)H * W + p];
+            }
+            const float dv = depth[p];
+            all_depth &= dv > 0.f;
+            d += dv;
+            if (render_mask) all_mask &= render_mask[p] != 0;
+        }
+    }
+    const size_t HWs = (size_t)Hs * Ws;
+    color_out[idx] = c0 / n_block;
+    color_out[HWs + idx] = c1 / n_block;
+    color_out[2 * HWs + idx] = c2 / n_block;
+    depth_out[idx] = all_depth ? d / n_block : 0.f;
+    if (render_mask) mask_out[idx] = all_mask ? 1 : 0;
+    if (tile_mask) {
+        const int ftx = (W + RTG_TILE - 1) / RTG_TILE, fty = (H + RTG_TILE - 1) / RTG_TILE;
+        const int ctx = (Ws + RTG_TILE - 1) / RTG_TILE, cty = (Hs + RTG_TILE - 1) / RTG_TILE;
+        if (idx < ctx * cty) {
+            const int tx = idx % ctx, ty = idx / ctx;
+            int any = 0;
+            for (int y = s * ty; y < min(s * ty + s, fty); y++)
+                for (int x = s * tx; x < min(s * tx + s, ftx); x++) any |= tile_mask[(size_t)y * ftx + x] != 0;
+            tile_mask_out[idx] = any;
+        }
+    }
+}
+
+void launch_frame_downsample(const float *color, const float *depth, const uint8_t *render_mask, const int32_t *tile_mask, int H,
+                             int W, int scale, int channels_last, float *color_out, float *depth_out, uint8_t *mask_out,
+                             int32_t *tile_mask_out, cudaStream_t s) {
+    const int n = (H / scale) * (W / scale);
+    frame_downsample_kernel<<<(n + 255) / 256, 256, 0, s>>>(color, depth, render_mask, tile_mask, H, W, scale, channels_last,
+                                                            color_out, depth_out, mask_out, tile_mask_out);
+}
+
 void launch_icp_build_level(const float *depth, int H, int W, int pool, float fx, float fy, float cx, float cy, float *vertex,
                             float *normal, void *ws_, cudaStream_t s);  // icp.cu
 

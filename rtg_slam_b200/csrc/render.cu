@@ -762,7 +762,11 @@ __global__ void BWD_BOUNDS render_bwd_kernel(const ViewParams vp, const GeomStat
 //   TAN_NORMAL_EQ: the residuals against the frame and the pixel selection of rtg_loss_l1, summed per tile into the
 //                  RTG_GN_ALL Gauss-Newton terms (warp butterfly in double, warps in order, one row per TILE ID so that
 //                  the launch order, which varies between runs, does not change any sum). No atomics.
-enum { TAN_IMAGES = 0, TAN_NORMAL_EQ = 1 };
+//   TAN_NORMAL_EQ_ROBUST: the same rows for the Huber objective by iteratively reweighted least squares: each residual r
+//                  (a colour channel, or the depth) gets the weight w = 1 for |r| <= delta, delta / |r| otherwise, in
+//                  float from the float residual; the rows hold (w J_a) J_c and (w J_a) r, and the two residual-square
+//                  terms hold sum 2 rho(r) (= sum r^2 while no |r| exceeds delta), so pose_gn_step_kernel is reused as is.
+enum { TAN_IMAGES = 0, TAN_NORMAL_EQ = 1, TAN_NORMAL_EQ_ROBUST = 2 };
 struct GnInputs {
     const float *render, *depth, *gt_color, *gt_depth;
     const uint8_t *mask;
@@ -771,15 +775,27 @@ struct GnInputs {
     double *partial;  // [tiles][RTG_GN_ALL]
 };
 
+// 2 rho(r) of the Huber loss: r^2 inside the threshold, delta (2 |r| - delta) outside
+__device__ __forceinline__ float huber2(const float r, const float delta) {
+    const float a = fabsf(r);
+    return a <= delta ? r * r : delta * (2.f * a - delta);
+}
+__device__ __forceinline__ float huber_weight(const float r, const float delta) {
+    const float a = fabsf(r);
+    return a <= delta ? 1.f : delta / a;
+}
+
+// The body of both kernel signatures below; `huber` (colour, depth thresholds) is read by TAN_NORMAL_EQ_ROBUST only.
 template <int MODE>
-__global__ void __launch_bounds__(256) render_tangent_kernel(const ViewParams vp, const GeomState g, const BinState b, const ImgState img,
-                                                             const int *__restrict__ counters, const int *__restrict__ hit_image,
-                                                             const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs in) {
+__device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                                                    const int *__restrict__ counters, const int *__restrict__ hit_image,
+                                                    const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs &in,
+                                                    const float2 huber) {
     __shared__ float4 s_s0[BATCH], s_s1[BATCH], s_rgb[BATCH];
     __shared__ int s_id[BATCH];
     __shared__ uint32_t s_mask[BATCH];
     __shared__ uint32_t s_max[8];
-    __shared__ double s_red[MODE == TAN_NORMAL_EQ ? 8 : 1][RTG_GN_ALL];
+    __shared__ double s_red[MODE != TAN_IMAGES ? 8 : 1][RTG_GN_ALL];
 
     const int tile = (int)b.active[blockIdx.x];
     int px, py;
@@ -907,21 +923,40 @@ __global__ void __launch_bounds__(256) render_tangent_kernel(const ViewParams vp
         }
         float v[RTG_GN_ALL];
         int q = 0;
+        if constexpr (MODE == TAN_NORMAL_EQ) {
 #pragma unroll
-        for (int a = 0; a < 6; a++)
+            for (int a = 0; a < 6; a++)
 #pragma unroll
-            for (int c = a; c < 6; c++, q++) {
-                v[q] = sc ? dC[0][a] * dC[0][c] + dC[1][a] * dC[1][c] + dC[2][a] * dC[2][c] : 0.f;
-                v[RTG_GN_TERMS + q] = sd ? dD[a] * dD[c] : 0.f;
+                for (int c = a; c < 6; c++, q++) {
+                    v[q] = sc ? dC[0][a] * dC[0][c] + dC[1][a] * dC[1][c] + dC[2][a] * dC[2][c] : 0.f;
+                    v[RTG_GN_TERMS + q] = sd ? dD[a] * dD[c] : 0.f;
+                }
+#pragma unroll
+            for (int a = 0; a < 6; a++) {
+                v[21 + a] = sc ? dC[0][a] * rc[0] + dC[1][a] * rc[1] + dC[2][a] * rc[2] : 0.f;
+                v[RTG_GN_TERMS + 21 + a] = sd ? dD[a] * rd : 0.f;
             }
+            v[27] = sc ? rc[0] * rc[0] + rc[1] * rc[1] + rc[2] * rc[2] : 0.f;
+            v[RTG_GN_TERMS + 27] = sd ? rd * rd : 0.f;
+        } else {
+            // a weight of 1 leaves w J_a bit-equal to J_a, so an unweighted pixel's terms are those of TAN_NORMAL_EQ
+            const float w0 = huber_weight(rc[0], huber.x), w1 = huber_weight(rc[1], huber.x), w2 = huber_weight(rc[2], huber.x);
+            const float wd = huber_weight(rd, huber.y);
 #pragma unroll
-        for (int a = 0; a < 6; a++) {
-            v[21 + a] = sc ? dC[0][a] * rc[0] + dC[1][a] * rc[1] + dC[2][a] * rc[2] : 0.f;
-            v[RTG_GN_TERMS + 21 + a] = sd ? dD[a] * rd : 0.f;
+            for (int a = 0; a < 6; a++) {
+                const float ja0 = w0 * dC[0][a], ja1 = w1 * dC[1][a], ja2 = w2 * dC[2][a], jd = wd * dD[a];
+#pragma unroll
+                for (int c = a; c < 6; c++, q++) {
+                    v[q] = sc ? ja0 * dC[0][c] + ja1 * dC[1][c] + ja2 * dC[2][c] : 0.f;
+                    v[RTG_GN_TERMS + q] = sd ? jd * dD[c] : 0.f;
+                }
+                v[21 + a] = sc ? ja0 * rc[0] + ja1 * rc[1] + ja2 * rc[2] : 0.f;
+                v[RTG_GN_TERMS + 21 + a] = sd ? jd * rd : 0.f;
+            }
+            v[27] = sc ? huber2(rc[0], huber.x) + huber2(rc[1], huber.x) + huber2(rc[2], huber.x) : 0.f;
+            v[RTG_GN_TERMS + 27] = sd ? huber2(rd, huber.y) : 0.f;
         }
-        v[27] = sc ? rc[0] * rc[0] + rc[1] * rc[1] + rc[2] * rc[2] : 0.f;
         v[28] = sc ? 1.f : 0.f;
-        v[RTG_GN_TERMS + 27] = sd ? rd * rd : 0.f;
         v[RTG_GN_TERMS + 28] = sd ? 1.f : 0.f;
 #pragma unroll
         for (int t = 0; t < RTG_GN_ALL; t++) {
@@ -938,6 +973,24 @@ __global__ void __launch_bounds__(256) render_tangent_kernel(const ViewParams vp
             in.partial[(size_t)tile * RTG_GN_ALL + threadIdx.x] = acc;
         }
     }
+}
+
+// Two signatures, so that TAN_IMAGES and TAN_NORMAL_EQ keep their parameter list (and their code) and only the robust
+// instantiation carries the Huber thresholds.
+template <int MODE>
+__global__ void __launch_bounds__(256) render_tangent_kernel(const ViewParams vp, const GeomState g, const BinState b, const ImgState img,
+                                                             const int *__restrict__ counters, const int *__restrict__ hit_image,
+                                                             const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs in) {
+    static_assert(MODE != TAN_NORMAL_EQ_ROBUST, "the robust rows take the Huber thresholds");
+    render_tangent_body<MODE>(vp, g, b, img, counters, hit_image, tan, J, in, make_float2(0.f, 0.f));
+}
+template <int MODE>
+__global__ void __launch_bounds__(256) render_tangent_kernel(const ViewParams vp, const GeomState g, const BinState b, const ImgState img,
+                                                             const int *__restrict__ counters, const int *__restrict__ hit_image,
+                                                             const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs in,
+                                                             const float2 huber) {
+    static_assert(MODE == TAN_NORMAL_EQ_ROBUST, "only the robust rows take the Huber thresholds");
+    render_tangent_body<MODE>(vp, g, b, img, counters, hit_image, tan, J, in, huber);
 }
 
 // One block: the fixed-order sum of the tiles' rows (one warp per term, fixed lane stride, fixed butterfly), then on one
@@ -1008,11 +1061,15 @@ void launch_render_tangent_images(const ViewParams &vp, int P, const GeomState &
 }
 
 void launch_pose_gn_normal_eq_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
-                                   const int32_t *counters, const RtgPoseGN &st, cudaStream_t s) {
+                                   const int32_t *counters, const RtgPoseGN &st, const RtgPoseRobust &robust, cudaStream_t s) {
     const int T = vp.tiles_x * vp.tiles_y;
     GnInputs in{st.render, st.depth, st.gt_color, st.gt_depth, st.render_mask, st.gt_channels_last, st.depth_error_max,
                 gn_partial(st.scratch, P)};
-    render_tangent_kernel<TAN_NORMAL_EQ><<<T, 256, 0, s>>>(vp, g, b, img, counters, st.hit_depth, tan_rows(st.scratch), nullptr, in);
+    if (robust.kernel == RTG_ROBUST_HUBER)
+        render_tangent_kernel<TAN_NORMAL_EQ_ROBUST><<<T, 256, 0, s>>>(vp, g, b, img, counters, st.hit_depth, tan_rows(st.scratch),
+                                                                     nullptr, in, make_float2(robust.color_delta, robust.depth_delta));
+    else
+        render_tangent_kernel<TAN_NORMAL_EQ><<<T, 256, 0, s>>>(vp, g, b, img, counters, st.hit_depth, tan_rows(st.scratch), nullptr, in);
     pose_gn_step_kernel<<<1, 256, 0, s>>>(T, in.partial, counters, st);
 }
 

@@ -21,13 +21,15 @@ again (the pose and Adam's state are untouched by the failed attempt).
 `PoseRefiner.refine_gn` minimises the squared colour + depth residuals over the same pixels by damped Gauss-Newton: per
 iteration the forward, then rtg_splat_pose_gn_step, which computes the forward-mode tangents of the render along the six
 twist directions, forms and solves the 6x6 normal equations and updates the pose, all on the device. `pose_jacobian`
-returns those tangent images themselves.
+returns those tangent images themselves. Optionally it runs coarse to fine over an image pyramid (`downsample_frame`,
+`level_camera`) and weighs each residual by the Huber loss (rtg_splat_pose_gn_step_robust).
 
 When to track with either (every frame, after ICP, on keyframes only) is SLAM policy and is left to the caller."""
 from __future__ import annotations
 
 import ctypes as C
 import math
+import types
 
 import torch
 
@@ -77,16 +79,95 @@ def pose_jacobian(raster_settings, means3D, opacities, shs=None, colors_precomp=
         return outs, J
 
 
+def level_camera(camera, s):
+    """The camera of pyramid level `s` (an integer >= 1) of `camera`, for images made by `downsample_frame`: the
+    Camera-like object PoseRefiner reads (world_view_transform, projection_matrix, FoVx, FoVy, image_height, image_width,
+    cx, cy). The rasterizer samples integer pixel coordinates (pixel = fx x / z + cx, fx = W / (2 tanfovx)), so coarse
+    pixel i looks along the ray of the fine block centre s i + (s - 1) / 2: with W_s = W // s,
+      fx_s = fx / s,  tanfovx_s = tanfovx s W_s / W,  cx_s = (cx - (s - 1) / 2) / s,
+    projection_matrix[0][0] scaled by W / (s W_s) (float64; the z rows unchanged), and likewise in y with H, H_s, cy.
+    The pose is shared with `camera`."""
+    s = int(s)
+    W, H = int(camera.image_width), int(camera.image_height)
+    if s < 1 or W // s < 1 or H // s < 1:
+        raise ValueError(f"there is no level {s} of a {W}x{H} camera")
+    Ws, Hs = W // s, H // s
+    projection = camera.projection_matrix.detach().to(torch.float64).clone()
+    projection[0, 0] *= W / (s * Ws)
+    projection[1, 1] *= H / (s * Hs)
+    return types.SimpleNamespace(
+        world_view_transform=camera.world_view_transform, projection_matrix=projection,
+        FoVx=2 * math.atan(math.tan(camera.FoVx * 0.5) * s * Ws / W), FoVy=2 * math.atan(math.tan(camera.FoVy * 0.5) * s * Hs / H),
+        image_width=Ws, image_height=Hs, cx=(camera.cx - (s - 1) / 2) / s, cy=(camera.cy - (s - 1) / 2) / s)
+
+
+def downsample_frame(gt_color, gt_depth, s, render_mask=None, tile_mask=None):
+    """Level `s` (>= 2) of a measured frame, in one launch of rtg_frame_downsample. gt_depth (H, W) or (1, H, W) float32
+    sets the size; gt_color (3, H, W) or (H, W, 3) float32; render_mask (H, W), any dtype, nonzero = selected; tile_mask
+    the rasterizer's int32 (ceil(H/16), ceil(W/16)) tile mask. All on one CUDA device. Returns (color (3, H_s, W_s),
+    depth (H_s, W_s), mask (H_s, W_s) uint8 or None, tile_mask (ceil(H_s/16), ceil(W_s/16)) int32 or None) with
+    H_s = H // s, W_s = W // s: colour is the block mean, depth the block mean where all s^2 depths are > 0 (else 0), the
+    render mask set where all s^2 pixels are set, a coarse tile set where any of its s x s fine tiles is set."""
+    s = int(s)
+    if s < 2:
+        raise ValueError("s must be >= 2")
+    H, W = int(gt_depth.shape[-2]), int(gt_depth.shape[-1])
+    if gt_depth.numel() != H * W:
+        raise ValueError("gt_depth must be (H,W) or (1,H,W)")
+    if gt_color.shape == (H, W, 3):
+        channels_last = 1
+    elif gt_color.shape == (3, H, W):
+        channels_last = 0
+    else:
+        raise ValueError("gt_color must be (H,W,3) or (3,H,W)")
+    for name, t in (("gt_color", gt_color), ("gt_depth", gt_depth)):
+        if not t.is_cuda or t.dtype != torch.float32:
+            raise TypeError(f"{name} must be a CUDA float32 tensor")
+    dev = gt_depth.device
+    Hs, Ws = H // s, W // s
+    gt_color, gt_depth = gt_color.detach().contiguous(), gt_depth.detach().contiguous()
+    color = torch.empty((3, Hs, Ws), dtype=torch.float32, device=dev)
+    depth = torch.empty((Hs, Ws), dtype=torch.float32, device=dev)
+    mask = mask_out = tmask = tmask_out = None
+    if render_mask is not None:
+        if render_mask.numel() != H * W:
+            raise ValueError("render_mask must have H*W elements")
+        mask = render_mask.detach().to(device=dev, dtype=torch.uint8).contiguous()
+        mask_out = torch.empty_like(depth, dtype=torch.uint8)
+    if tile_mask is not None:
+        if not tile_mask.is_cuda or tile_mask.dtype != torch.int32:
+            raise TypeError("tile_mask must be a CUDA int32 tensor")
+        if tile_mask.numel() != ((H + 15) // 16) * ((W + 15) // 16):
+            raise ValueError(f"tile_mask must have {(H + 15) // 16}x{(W + 15) // 16} entries")
+        tmask = tile_mask.contiguous()
+        tmask_out = torch.empty(((Hs + 15) // 16, (Ws + 15) // 16), dtype=torch.int32, device=dev)
+    p = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+    check(_lib.lib().rtg_frame_downsample(p(gt_color), p(gt_depth), p(mask), p(tmask), H, W, s, channels_last, p(color), p(depth),
+                                          p(mask_out), p(tmask_out), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+          "rtg_frame_downsample")
+    return color, depth, mask_out, tmask_out
+
+
 class PoseRefiner:
     """Refines a world-to-camera pose against a frozen Gaussian map. `args` is the bag `render.Renderer` takes."""
 
     def __init__(self, args):
         self._renderer = Renderer(args)  # rasterizer settings exactly as Renderer.render makes them
 
+    def _settings(self, camera, dev, view, proj, campos):
+        """Rasterizer settings at `camera`'s image size and intrinsics over the three camera tensors."""
+        r = self._renderer
+        return GaussianRasterizationSettings(
+            image_height=int(camera.image_height), image_width=int(camera.image_width),
+            tanfovx=math.tan(camera.FoVx * 0.5), tanfovy=math.tan(camera.FoVy * 0.5), bg=r.bg_color.to(dev),
+            scale_modifier=r.scaling_modifier, viewmatrix=view, projmatrix=proj, sh_degree=r.active_sh_degree, campos=campos,
+            opaque_threshold=r.renderer_opaque_threshold, depth_threshold=r.renderer_depth_threshold,
+            normal_threshold=r.renderer_normal_threshold, color_sigma=r.color_sigma, prefiltered=False, debug=False,
+            cx=camera.cx, cy=camera.cy, T_threshold=0.0001)
+
     def _setup(self, camera, gaussian_data, requires_grad):
         """The double pose W2C, the projection, the three camera tensors the rasterizer reads (rewritten in place by the
         device pose steps), the rasterizer settings over them and the detached map."""
-        r = self._renderer
         dev = gaussian_data["xyz"].device
         vm0 = camera.world_view_transform.detach().to(device=dev, dtype=torch.float64)
         pose = vm0.t().contiguous()                                   # W2C, row-major, double
@@ -94,18 +175,13 @@ class PoseRefiner:
         view = pose.t().float().contiguous().requires_grad_(requires_grad)
         proj = (pose.t() @ projection.double()).float().contiguous().requires_grad_(requires_grad)
         campos = (-(pose[:3, :3].t() @ pose[:3, 3])).float().contiguous().requires_grad_(requires_grad)
-        rs = GaussianRasterizationSettings(
-            image_height=int(camera.image_height), image_width=int(camera.image_width),
-            tanfovx=math.tan(camera.FoVx * 0.5), tanfovy=math.tan(camera.FoVy * 0.5), bg=r.bg_color.to(dev),
-            scale_modifier=r.scaling_modifier, viewmatrix=view, projmatrix=proj, sh_degree=r.active_sh_degree, campos=campos,
-            opaque_threshold=r.renderer_opaque_threshold, depth_threshold=r.renderer_depth_threshold,
-            normal_threshold=r.renderer_normal_threshold, color_sigma=r.color_sigma, prefiltered=False, debug=False,
-            cx=camera.cx, cy=camera.cy, T_threshold=0.0001)
+        rs = self._settings(camera, dev, view, proj, campos)
         g = {k: gaussian_data[k].detach() for k in ("xyz", "opacity", "shs", "scales", "rotations")}
         return dev, pose, projection, view, proj, campos, rs, g
 
     def refine_gn(self, camera, gaussian_data, gt_color, gt_depth, iters, damping=1e-4, color_weight=0.8, depth_weight=1.0,
-                  render_mask=None, tile_mask=None, depth_error_max=0.1):
+                  render_mask=None, tile_mask=None, depth_error_max=0.1, scales=(1,), robust=None, color_delta=0.1,
+                  depth_delta=0.05):
         """Gauss-Newton refinement of the pose on the squared colour + depth residuals (rtg_splat_pose_gn_step): per
         iteration the rasterizer forward, then the forward-mode tangents of the render along the six twist directions, the
         normal equations over rtg_loss_l1's pixel selection, the damped solve (H + damping * trace(H) * I) and
@@ -113,13 +189,28 @@ class PoseRefiner:
         that each iteration waits for its forward's scan kernel: an iteration whose render overflowed the binning buffer is
         rendered again (with the capacity raised), keeping the pose refined so far.
 
-        Arguments as in `refine`; `damping` scales the trace added to the diagonal. Returns (W2C, report): the refined pose,
-        a (4, 4) float64 CUDA tensor, and the last step's report, a float64 CUDA tensor [E, E_colour, E_depth, N_c, N_d,
-        |rho|, |phi|, status] (E evaluated before that step; status 0 ok, 1 singular system, 2 no selected pixel,
-        3 overflowed forward -- the pose is then left unchanged)."""
-        iters = int(iters)
-        if iters < 1:
+        Arguments as in `refine`; `damping` scales the trace added to the diagonal.
+        `scales`: the image pyramid, decreasing and ending in 1, e.g. (4, 2, 1). Level s renders at `level_camera(camera,
+        s)` against `downsample_frame(...)` of the targets and masks (made once per call); level 1 uses the caller's
+        tensors. The pose carries over from level to level on the device. `iters`: one count for every level, or one per
+        entry of `scales`. A level whose selection is empty leaves the pose as it is and the next level goes on from it.
+        `robust`: None (squared residuals) or "huber" (rtg_splat_pose_gn_step_robust: Huber loss with thresholds
+        `color_delta` in colour units and `depth_delta` in map units, minimised by reweighted least squares).
+        The defaults (one level, no robust loss) run one rtg_splat_pose_gn_step per iteration and nothing else.
+
+        Returns (W2C, report): the refined pose, a (4, 4) float64 CUDA tensor, and the finest level's last step's report,
+        a float64 CUDA tensor [E, E_colour, E_depth, N_c, N_d, |rho|, |phi|, status] (E evaluated before that step; status
+        0 ok, 1 singular system, 2 no selected pixel, 3 overflowed forward -- the pose is then left unchanged)."""
+        scales = tuple(int(x) for x in scales)
+        if not scales or scales[-1] != 1 or any(a <= b for a, b in zip(scales, scales[1:])):
+            raise ValueError("scales must be decreasing and end in 1")
+        level_iters = [int(i) for i in iters] if isinstance(iters, (list, tuple)) else [int(iters)] * len(scales)
+        if len(level_iters) != len(scales):
+            raise ValueError("iters must be an int or one count per entry of scales")
+        if min(level_iters) < 1:
             raise ValueError("iters must be >= 1")
+        if robust not in (None, "huber"):
+            raise ValueError('robust must be None or "huber"')
         dev, pose, projection, view, proj, campos, rs, g = self._setup(camera, gaussian_data, requires_grad=False)
         H, W = int(rs.image_height), int(rs.image_width)
         gt_color, gt_depth = gt_color.detach().contiguous(), gt_depth.detach().contiguous()
@@ -141,29 +232,52 @@ class PoseRefiner:
                 raise ValueError("render_mask must have H*W elements")
         P = int(g["xyz"].shape[0])
         L = _lib.lib()
-        scratch = torch.empty((int(L.rtg_splat_pose_gn_scratch_bytes(P, H, W)),), dtype=torch.uint8, device=dev)
+        scratch = torch.empty((int(L.rtg_splat_pose_gn_scratch_bytes(P, H, W)),), dtype=torch.uint8, device=dev)  # the finest level's
         report = torch.zeros(_lib.RTG_POSE_GN_REPORT_LEN, dtype=torch.float64, device=dev)
-        s = RtgPoseGN()
-        s.pose, s.projection, s.viewmatrix, s.projmatrix, s.campos = (t.data_ptr() for t in (pose, projection, view, proj, campos))
-        s.gt_color, s.gt_depth = gt_color.data_ptr(), gt_depth.data_ptr()
-        s.render_mask = None if mask is None else mask.data_ptr()
-        s.scratch, s.report = scratch.data_ptr(), report.data_ptr()
-        s.color_weight, s.depth_weight, s.depth_error_max, s.damping = (float(color_weight), float(depth_weight),
-                                                                          float(depth_error_max), float(damping))
-        s.gt_channels_last = channels_last
+
+        def state(projection, gt_color, gt_depth, mask, channels_last):
+            s = RtgPoseGN()
+            s.pose, s.projection, s.viewmatrix, s.projmatrix, s.campos = (t.data_ptr() for t in (pose, projection, view, proj, campos))
+            s.gt_color, s.gt_depth = gt_color.data_ptr(), gt_depth.data_ptr()
+            s.render_mask = None if mask is None else mask.data_ptr()
+            s.scratch, s.report = scratch.data_ptr(), report.data_ptr()
+            s.color_weight, s.depth_weight, s.depth_error_max, s.damping = (float(color_weight), float(depth_weight),
+                                                                              float(depth_error_max), float(damping))
+            s.gt_channels_last = channels_last
+            return s
+
+        # per level: settings, projection, the step's state and the tile mask (the tensors are kept alive by `levels`)
+        levels = []
+        for sc in scales:
+            if sc == 1:
+                levels.append((rs, projection, state(projection, gt_color, gt_depth, mask, channels_last), tile_mask, None))
+                continue
+            cam = level_camera(camera, sc)
+            lproj = cam.projection_matrix.to(device=dev, dtype=torch.float32).contiguous()
+            targets = downsample_frame(gt_color, gt_depth.view(H, W), sc, mask, tile_mask)
+            levels.append((self._settings(cam, dev, view, proj, campos), lproj, state(lproj, *targets[:3], 0), targets[3], targets))
+        if robust is None:
+            step, extra = L.rtg_splat_pose_gn_step, ()
+        else:
+            r = _lib.RtgPoseRobust()
+            r.kernel, r.color_delta, r.depth_delta = _lib.RTG_ROBUST_HUBER, float(color_delta), float(depth_delta)
+            step, extra = L.rtg_splat_pose_gn_step_robust, (C.byref(r),)
         st = rasterizer._state(dev)
-        for _ in range(iters):
-            for attempt in range(2):
-                outs, saved, ins = _forward_native(rs, g["xyz"], g["shs"], None, g["opacity"], g["scales"], g["rotations"], None,
-                                                   tile_mask)
-                st.read(saved.pending, block=True)  # this forward's scan kernel; the capacity is raised on an overflow
-                if not saved.pending.overflow:
-                    break
-                if attempt:
-                    raise CapacityOverflow("PoseRefiner.refine_gn: the render overflowed the binning buffer twice")
-            s.render, s.depth, s.hit_depth = outs[0].data_ptr(), outs[1].data_ptr(), outs[3].data_ptr()
-            check(L.rtg_splat_pose_gn_step(*_native_args(rs, saved, ins, dev), C.byref(s),
-                                           C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "rtg_splat_pose_gn_step")
+        for (lrs, lproj, s, ltm, _), n in zip(levels, level_iters):
+            if len(levels) > 1:  # this level's projmatrix from the pose, on the device
+                proj.copy_((pose.t() @ lproj.double()).float())
+            for _ in range(n):
+                for attempt in range(2):
+                    outs, saved, ins = _forward_native(lrs, g["xyz"], g["shs"], None, g["opacity"], g["scales"], g["rotations"],
+                                                       None, ltm)
+                    st.read(saved.pending, block=True)  # this forward's scan kernel; the capacity is raised on an overflow
+                    if not saved.pending.overflow:
+                        break
+                    if attempt:
+                        raise CapacityOverflow("PoseRefiner.refine_gn: the render overflowed the binning buffer twice")
+                s.render, s.depth, s.hit_depth = outs[0].data_ptr(), outs[1].data_ptr(), outs[3].data_ptr()
+                check(step(*_native_args(lrs, saved, ins, dev), C.byref(s), *extra,
+                           C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), step.__name__)
         return pose, report
 
     def refine(self, camera, gaussian_data, gt_color, gt_depth, iters, lr_rot, lr_trans, color_weight=0.8, depth_weight=1.0,

@@ -343,6 +343,37 @@ int rtg_splat_pose_gn_step_robust(const RtgSplatView *view, int32_t P, int32_t M
                                   const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
                                   const RtgPoseGN *s, const RtgPoseRobust *robust, void *stream);
 
+/* rtg_splat_pose_gn_step_exposure: the step of rtg_splat_pose_gn_step_robust with the frame's exposure estimated with the
+ * pose. The camera's pixel values are modelled as C^ = e^a C + b (one gain and one offset per frame, shared by the three
+ * channels; (0, 0) = none), the colour residual of a selected pixel and channel is r = e^a C + b - C^, and with the
+ * unknowns x = (rho, phi, a, b) its Jacobian row is (e^a dC/dxi, e^a C, 1). Depth residuals, the pixel sets, the counts,
+ * the weights and the Huber rule are those of rtg_splat_pose_gn_step[_robust], applied to the new r:
+ *   E = 1/2 [ color_weight / N_c sum_{S_c} sum_ch r^2 + depth_weight / N_d sum_{S_d} (D - D^)^2 ]    (RTG_ROBUST_NONE)
+ *   E = color_weight / N_c sum_{S_c} sum_ch rho_cd(r) + depth_weight / N_d sum_{S_d} rho_dd(D - D^)     (RTG_ROBUST_HUBER)
+ * H (8x8, the depth block in its leading 6x6) and g are summed in double in a fixed order (identical inputs give
+ * bit-identical sums). Damping: the six pose diagonals get damping * trace(H[0:6, 0:6]), as rtg_splat_pose_gn_step's, so
+ * that the pose step with the exposure columns removed is that entry's; the exposure diagonals are scaled, H_aa (1 +
+ * damping) and H_bb (1 + damping): the pose trace is of order (focal length * image gradient)^2 while H_bb =
+ * color_weight, so adding it there would freeze the exposure. x = -H^-1 g; W2C <- exp(xi^) W2C, a += x_6, b += x_7 in
+ * double in `exposure->ab`, and the camera arrays are rewritten. `report` as rtg_splat_pose_gn_step's, E the objective
+ * with the exposure before the step.
+ * Degenerate cases: with N_c = 0 or color_weight = 0 the exposure columns are empty; the 6x6 pose system is solved alone,
+ * (a, b) is left unchanged and the status stays RTG_POSE_GN_OK. A singular system, N_c + N_d = 0 or an overflowed forward
+ * leaves the pose, the arrays and (a, b) unchanged.
+ * `s->scratch` holds rtg_splat_pose_gn_exposure_scratch_bytes(P, H, W) bytes (the tangent rows and RTG_GN_EXP_ALL = 75
+ * doubles per tile); rtg_splat_pose_gn_scratch_bytes keeps its value. `robust->kernel` may be RTG_ROBUST_NONE. Rejects a
+ * NULL `exposure`, a NULL or misaligned `ab` and everything rtg_splat_pose_gn_step_robust rejects, on the host before any
+ * CUDA work. */
+typedef struct RtgPoseExposure {
+    double *ab;                                         /* 2 doubles on the device: (a, b), updated in place by the step */
+} RtgPoseExposure;
+size_t rtg_splat_pose_gn_exposure_scratch_bytes(int32_t P, int32_t H, int32_t W);
+int rtg_splat_pose_gn_step_exposure(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                                    const float *colors_precomp, const float *scales, const float *rotations,
+                                    const float *cov3D_precomp, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                                    int64_t R_cap, const int32_t *counters, const RtgPoseGN *s, const RtgPoseRobust *robust,
+                                    const RtgPoseExposure *exposure, void *stream);
+
 /* Replaces CudaRasterizer::Rasterizer::markVisible (rasterizer.h:21-26, rasterizer_impl.cu:145-157). */
 int rtg_splat_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix,
                            uint8_t *present, void *stream);
@@ -499,6 +530,20 @@ size_t rtg_loss_workspace_bytes(void);
 int rtg_loss_l1(const float *render, const float *depth, const int32_t *depth_index, const float *gt_color, const float *gt_depth,
                 const uint8_t *render_mask, int32_t H, int32_t W, int32_t gt_channels_last, float color_weight, float depth_weight,
                 float depth_error_max, float *dL_dcolor, float *dL_ddepth, float *loss_out, void *ws, void *stream);
+
+/* rtg_loss_l1_exposure: rtg_loss_l1 of a render seen under a frame exposure (a, b) = `exposure` (2 device floats): the colour
+ * term is the mean of |r|, r = e^a render + b - gt_color, over the same pixels; the depth term is unchanged. Written:
+ *   dL_dcolor = color_weight / N_c e^a sgn(r),  dL_ddepth as rtg_loss_l1,
+ *   dL_dexposure (2 device floats) = color_weight / N_c (sum sgn(r) e^a render, sum sgn(r)),  N_c = 3 x selected pixels,
+ * and loss_out as rtg_loss_l1. exposure = (0, 0) gives rtg_loss_l1's loss and gradients. The sums are formed in double from
+ * per-block partial sums added in a fixed order (no atomics): identical inputs give bit-identical outputs.
+ * ws: rtg_loss_l1_exposure_workspace_bytes() bytes. Rejects a NULL pointer (render_mask may be NULL) and H, W <= 0 on the
+ * host before any CUDA work. */
+size_t rtg_loss_l1_exposure_workspace_bytes(void);
+int rtg_loss_l1_exposure(const float *render, const float *depth, const int32_t *depth_index, const float *gt_color,
+                         const float *gt_depth, const uint8_t *render_mask, int32_t H, int32_t W, int32_t gt_channels_last,
+                         float color_weight, float depth_weight, float depth_error_max, const float *exposure, float *dL_dcolor,
+                         float *dL_ddepth, float *dL_dexposure, float *loss_out, void *ws, void *stream);
 
 /* The same loss with the cosine normal term of Mapping.loss_update (mapper.py:433-442):
  *   normal = mean of 1 - cosine_similarity(render_normal, gt_normal) over pixels with render_mask, depth_index != -1 and

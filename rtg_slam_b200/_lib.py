@@ -85,6 +85,11 @@ class RtgPoseRobust(C.Structure):
 RTG_ROBUST_NONE, RTG_ROBUST_HUBER = 0, 1
 
 
+class RtgPoseExposure(C.Structure):
+    """include/rtg_splat_b200.h: RtgPoseExposure (field order is the ABI)."""
+    _fields_ = [("ab", C.c_void_p)]
+
+
 class RtgIcpLevel(C.Structure):
     _fields_ = [("vertex0", C.c_void_p), ("normal0", C.c_void_p), ("vertex1", C.c_void_p), ("normal1", C.c_void_p),
                 ("H", C.c_int32), ("W", C.c_int32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
@@ -123,6 +128,9 @@ SIGNATURES = {
                                + [C.POINTER(RtgPoseGN), _VP]),
     "rtg_splat_pose_gn_step_robust": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
                                       + [C.POINTER(RtgPoseGN), C.POINTER(RtgPoseRobust), _VP]),
+    "rtg_splat_pose_gn_exposure_scratch_bytes": (C.c_size_t, [_I32, _I32, _I32]),
+    "rtg_splat_pose_gn_step_exposure": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
+                                        + [C.POINTER(RtgPoseGN), C.POINTER(RtgPoseRobust), C.POINTER(RtgPoseExposure), _VP]),
     "rtg_splat_mark_visible": (C.c_int, [_I32, _VP, _VP, _VP, _VP, _VP]),
     "rtg_adam_step": (C.c_int, [C.POINTER(RtgAdamGroup), _I32, _F, _F, _F, _I32, _VP]),
     "rtg_map_adam_step": (C.c_int, [C.POINTER(RtgMapStep), _VP]),
@@ -137,6 +145,9 @@ SIGNATURES = {
     "rtg_icp_fill_model_depth": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _F, _F, _VP]),
     "rtg_loss_workspace_bytes": (C.c_size_t, []),
     "rtg_loss_l1": (C.c_int, [_VP] * 6 + [_I32, _I32, _I32, _F, _F, _F, _VP, _VP, _VP, _VP, _VP]),
+    # rtg_loss_l1's arguments with exposure before the gradients and dL_dexposure after them
+    "rtg_loss_l1_exposure_workspace_bytes": (C.c_size_t, []),
+    "rtg_loss_l1_exposure": (C.c_int, [_VP] * 6 + [_I32, _I32, _I32, _F, _F, _F, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "rtg_loss_mapping": (C.c_int, [_VP] * 8 + [_I32, _I32, _I32, _F, _F, _F, _F, _VP, _VP, _VP, _VP, _VP, _VP]),
     "rtg_ssim_workspace_bytes": (C.c_size_t, [_I32, _I32, _I32]),
     "rtg_ssim_loss": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _VP, _VP, _VP, _VP]),

@@ -17,6 +17,9 @@ int launch_adam(const RtgAdamGroup *groups, int n_groups, float beta1, float bet
 void launch_pose_adam_step(const RtgPoseAdam &st, cudaStream_t s);
 void launch_pose_gn_normal_eq_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
                                    const int32_t *counters, const RtgPoseGN &st, const RtgPoseRobust &robust, cudaStream_t s);
+void launch_pose_gn_exposure_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                  const int32_t *counters, const RtgPoseGN &st, const RtgPoseRobust &robust, double *ab,
+                                  cudaStream_t s);
 void launch_frame_downsample(const float *color, const float *depth, const uint8_t *render_mask, const int32_t *tile_mask, int H,
                              int W, int scale, int channels_last, float *color_out, float *depth_out, uint8_t *mask_out,
                              int32_t *tile_mask_out, cudaStream_t s);
@@ -43,6 +46,11 @@ void launch_loss_mapping(const float *render, const float *depth, const float *r
                          const float *gt_color, const float *gt_depth, const float *gt_normal, const uint8_t *mask, int H, int W,
                          int channels_last, float color_weight, float depth_weight, float normal_weight, float depth_error_max,
                          float *dL_dcolor, float *dL_ddepth, float *dL_dnormal, float *loss_out, void *ws, cudaStream_t s);
+size_t loss_exposure_ws_bytes();
+void launch_loss_l1_exposure(const float *render, const float *depth, const int *depth_index, const float *gt_color,
+                             const float *gt_depth, const uint8_t *mask, int H, int W, int channels_last, float color_weight,
+                             float depth_weight, float depth_error_max, const float *exposure, float *dL_dcolor, float *dL_ddepth,
+                             float *dL_dexposure, float *loss_out, void *ws, cudaStream_t s);
 void launch_normal_map(const float *normal, const int *depth_index, int H, int W, float *out, cudaStream_t s);
 void launch_icp_fill(float *render_depth, const float *frame_depth, const float *rn, const float *fn, int H, int W, float dthr,
                      float nthr, cudaStream_t s);
@@ -569,11 +577,12 @@ int rtg_splat_pose_tangents(const RtgSplatView *view, int32_t P, int32_t M, cons
     return check_launch(who);
 }
 
-// The step of both Gauss-Newton entry points: `robust` selects the normal-equation rows (RTG_ROBUST_NONE: the plain ones).
+// The step of the Gauss-Newton entry points: `robust` selects the normal-equation rows (RTG_ROBUST_NONE: the plain ones),
+// `ab` (the device exposure, or nullptr) the eight-unknown step.
 static int pose_gn_step(const char *who, const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
                         const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
                         const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
-                        const RtgPoseGN *st, const RtgPoseRobust &robust, void *stream) {
+                        const RtgPoseGN *st, const RtgPoseRobust &robust, double *ab, void *stream) {
     int rc = validate_pose_tangent_inputs(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws,
                                           img_ws, bin_ws, R_cap, counters, st->hit_depth, st->scratch);
     if (rc) return rc;
@@ -593,7 +602,8 @@ static int pose_gn_step(const char *who, const RtgSplatView *view, int32_t P, in
     rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
     rtg::launch_preprocess_tangent(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count,
                                    reinterpret_cast<float4 *>(st->scratch), s);
-    rtg::launch_pose_gn_normal_eq_step(vp, P, g, b, img, counters, *st, robust, s);
+    if (ab) rtg::launch_pose_gn_exposure_step(vp, P, g, b, img, counters, *st, robust, ab, s);
+    else rtg::launch_pose_gn_normal_eq_step(vp, P, g, b, img, counters, *st, robust, s);
     return check_launch(who);
 }
 
@@ -605,14 +615,10 @@ int rtg_splat_pose_gn_step(const RtgSplatView *view, int32_t P, int32_t M, const
     if (!st) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": state is NULL");
     const RtgPoseRobust none{RTG_ROBUST_NONE, 0.f, 0.f, 0};
     return pose_gn_step(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws, img_ws, bin_ws,
-                        R_cap, counters, st, none, stream);
+                        R_cap, counters, st, none, nullptr, stream);
 }
 
-int rtg_splat_pose_gn_step_robust(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
-                                  const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
-                                  const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
-                                  const RtgPoseGN *st, const RtgPoseRobust *robust, void *stream) {
-    const char *who = "rtg_splat_pose_gn_step_robust";
+static int validate_pose_robust(const char *who, const RtgPoseGN *st, const RtgPoseRobust *robust) {
     if (!st) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": state is NULL");
     if (!robust) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": robust is NULL");
     if (robust->kernel != RTG_ROBUST_NONE && robust->kernel != RTG_ROBUST_HUBER)
@@ -621,8 +627,37 @@ int rtg_splat_pose_gn_step_robust(const RtgSplatView *view, int32_t P, int32_t M
         !(std::isfinite(robust->color_delta) && robust->color_delta > 0.f && std::isfinite(robust->depth_delta) &&
           robust->depth_delta > 0.f))
         return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": color_delta and depth_delta must be positive and finite");
+    return RTG_OK;
+}
+
+int rtg_splat_pose_gn_step_robust(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                                  const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
+                                  const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
+                                  const RtgPoseGN *st, const RtgPoseRobust *robust, void *stream) {
+    const char *who = "rtg_splat_pose_gn_step_robust";
+    int rc = validate_pose_robust(who, st, robust);
+    if (rc) return rc;
     return pose_gn_step(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws, img_ws, bin_ws,
-                        R_cap, counters, st, *robust, stream);
+                        R_cap, counters, st, *robust, nullptr, stream);
+}
+
+size_t rtg_splat_pose_gn_exposure_scratch_bytes(int32_t P, int32_t H, int32_t W) {
+    return (P < 0 || H <= 0 || W <= 0) ? 0 : rtg::pose_gn_exposure_scratch_bytes(P, H, W);
+}
+
+int rtg_splat_pose_gn_step_exposure(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                                    const float *colors_precomp, const float *scales, const float *rotations,
+                                    const float *cov3D_precomp, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                                    int64_t R_cap, const int32_t *counters, const RtgPoseGN *st, const RtgPoseRobust *robust,
+                                    const RtgPoseExposure *exposure, void *stream) {
+    const char *who = "rtg_splat_pose_gn_step_exposure";
+    int rc = validate_pose_robust(who, st, robust);
+    if (rc) return rc;
+    if (!exposure) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": exposure is NULL");
+    if (!exposure->ab) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": exposure ab is NULL");
+    if (((uintptr_t)exposure->ab) & 7) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": exposure ab must be 8-byte aligned");
+    return pose_gn_step(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws, img_ws, bin_ws,
+                        R_cap, counters, st, *robust, exposure->ab, stream);
 }
 
 int rtg_pose_adam_step(const RtgPoseAdam *st, void *stream) {
@@ -808,6 +843,24 @@ int rtg_loss_l1(const float *render, const float *depth, const int32_t *depth_in
     rtg::launch_loss_l1(render, depth, depth_index, gt_color, gt_depth, render_mask, H, W, gt_channels_last, color_weight, depth_weight,
                         depth_error_max, dL_dcolor, dL_ddepth, loss_out, ws, reinterpret_cast<cudaStream_t>(stream));
     return check_launch("rtg_loss_l1");
+}
+
+size_t rtg_loss_l1_exposure_workspace_bytes(void) { return rtg::loss_exposure_ws_bytes(); }
+
+int rtg_loss_l1_exposure(const float *render, const float *depth, const int32_t *depth_index, const float *gt_color,
+                         const float *gt_depth, const uint8_t *render_mask, int32_t H, int32_t W, int32_t gt_channels_last,
+                         float color_weight, float depth_weight, float depth_error_max, const float *exposure, float *dL_dcolor,
+                         float *dL_ddepth, float *dL_dexposure, float *loss_out, void *ws, void *stream) {
+    const char *who = "rtg_loss_l1_exposure";
+    if (H <= 0 || W <= 0) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": H and W must be >= 1");
+    if (!render || !depth || !depth_index || !gt_color || !gt_depth || !dL_dcolor || !dL_ddepth || !loss_out || !ws)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pointer");
+    if (!exposure || !dL_dexposure) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL exposure / dL_dexposure");
+    if (((uintptr_t)ws) & 7) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": ws must be 8-byte aligned");
+    rtg::launch_loss_l1_exposure(render, depth, depth_index, gt_color, gt_depth, render_mask, H, W, gt_channels_last, color_weight,
+                                 depth_weight, depth_error_max, exposure, dL_dcolor, dL_ddepth, dL_dexposure, loss_out, ws,
+                                 reinterpret_cast<cudaStream_t>(stream));
+    return check_launch(who);
 }
 
 int rtg_loss_mapping(const float *render, const float *depth, const float *render_normal, const int32_t *depth_index,

@@ -26,6 +26,10 @@ enum { REC_COLOR = 0, REC_M0 = 3, REC_MX = 4, REC_MY = 5, REC_MXX = 6, REC_MXY =
 // sum r^2, pixel count. The colour set comes first, then the depth set.
 #define RTG_GN_TERMS 29
 #define RTG_GN_ALL (2 * RTG_GN_TERMS)
+// The same with the frame's exposure (a, b) as unknowns 6 and 7 of the colour set: 36 entries of the 8x8 J^T J (upper
+// triangle, row by row), 8 of J^T r, sum 2 rho(r), pixel count. The depth set keeps its RTG_GN_TERMS and follows.
+#define RTG_GN_EXP_COLOR 46
+#define RTG_GN_EXP_ALL (RTG_GN_EXP_COLOR + RTG_GN_TERMS)
 
 struct ViewParams {
     int H, W, tiles_x, tiles_y;
@@ -368,6 +372,47 @@ __device__ __forceinline__ bool solve6(const double A[6][6], const double bvec[6
         double v = y[i];
 #pragma unroll
         for (int k = i + 1; k < 6; k++) v -= Lm[k][i] * x[k];
+        x[i] = v / Lm[i][i];
+    }
+    return ok;
+}
+
+// solve6's Cholesky for an N x N symmetric positive definite system (the 8 unknowns of the pose step with exposure). A
+// separate function: solve6 and the kernels that call it keep their code.
+template <int N>
+__device__ __forceinline__ bool solve_n(const double A[N][N], const double bvec[N], double x[N]) {
+    double Lm[N][N];
+    bool ok = true;
+#pragma unroll
+    for (int j = 0; j < N; j++) {
+        double d = A[j][j];
+#pragma unroll
+        for (int k = 0; k < j; k++) d -= Lm[j][k] * Lm[j][k];
+        ok = ok && (d > 0.0);
+        const double ljj = sqrt(fmax(d, 1e-300));
+        Lm[j][j] = ljj;
+        const double inv = 1.0 / ljj;
+#pragma unroll
+        for (int i = j + 1; i < N; i++) {
+            double v = A[i][j];
+#pragma unroll
+            for (int k = 0; k < j; k++) v -= Lm[i][k] * Lm[j][k];
+            Lm[i][j] = v * inv;
+        }
+    }
+    double y[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+        double v = bvec[i];
+#pragma unroll
+        for (int k = 0; k < i; k++) v -= Lm[i][k] * y[k];
+        y[i] = v / Lm[i][i];
+    }
+#pragma unroll
+    for (int i = N - 1; i >= 0; i--) {
+        double v = y[i];
+#pragma unroll
+        for (int k = i + 1; k < N; k++) v -= Lm[k][i] * x[k];
         x[i] = v / Lm[i][i];
     }
     return ok;

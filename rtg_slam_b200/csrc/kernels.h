@@ -51,6 +51,7 @@ void launch_render_bwd(const ViewParams &vp, const GeomState &g, const BinState 
                        cudaStream_t s, const float *dL_dT = nullptr);  // dL_dT: (H, W) dL/dT_map, or NULL
 // pose Gauss-Newton: scratch = the tangent rows (read) and the per-tile partial sums
 size_t pose_gn_scratch_bytes(int P, int H, int W);
+size_t pose_gn_exposure_scratch_bytes(int P, int H, int W);  // the per-tile rows hold RTG_GN_EXP_ALL terms
 void launch_render_tangent_images(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
                                   const int32_t *counters, const int *hit_image, void *scratch, float *J, cudaStream_t s);
 

@@ -93,6 +93,121 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(const float *__restrict_
     }
 }
 
+// ---- the L1 loss under a frame exposure (a, b): the colour residual is r = e^a C + b - C^, the depth term is unchanged.
+// Besides the four statistics, sum sgn(r) e^a C and sum sgn(r) give dL/da and dL/db. Every block writes its six partial
+// sums (no atomics); one block adds them in a fixed order, so two calls on the same inputs give the same bits.
+#define RTG_LOSS_EXP_TERMS 6
+struct LossExposureWs {
+    LossStats st;
+    double partial[RTG_NUM_SMS * 8][RTG_LOSS_EXP_TERMS];
+};
+
+__global__ void __launch_bounds__(256) loss_exposure_reduce_kernel(const float *__restrict__ render, const float *__restrict__ depth,
+                                                                   const int *__restrict__ depth_index,
+                                                                   const float *__restrict__ gt_color,
+                                                                   const float *__restrict__ gt_depth, const uint8_t *__restrict__ mask,
+                                                                   int N, int channels_last, float depth_error_max,
+                                                                   const float *__restrict__ exposure, LossExposureWs *ws) {
+    const float ea = expf(exposure[0]), eb = exposure[1];
+    double a[RTG_LOSS_EXP_TERMS] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < N; p += gridDim.x * blockDim.x) {
+        const bool m = mask ? (mask[p] != 0) : true;
+        if (m) {
+            float s = 0.f, sa = 0.f, sb = 0.f;
+#pragma unroll
+            for (int c = 0; c < 3; c++) {
+                const float g = channels_last ? gt_color[3 * (size_t)p + c] : gt_color[(size_t)c * N + p];
+                const float C = render[(size_t)c * N + p], ec = ea * C;
+                const float r = fmaf(ea, C, eb) - g;  // the expression of loss_exposure_grad_kernel
+                s += fabsf(r);
+                sa += sgn(r) * ec;
+                sb += sgn(r);
+            }
+            a[0] += (double)s;
+            a[1] += 1.0;
+            a[4] += (double)sa;
+            a[5] += (double)sb;
+            const float gd = gt_depth[p];
+            const float e = depth[p] - gd;
+            if (depth_index[p] != -1 && gd > 0.f && e < depth_error_max) { a[2] += (double)fabsf(e); a[3] += 1.0; }
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < RTG_LOSS_EXP_TERMS; k++)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a[k] += __shfl_xor_sync(0xffffffffu, a[k], o);
+    __shared__ double s_p[8][RTG_LOSS_EXP_TERMS];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < RTG_LOSS_EXP_TERMS; k++) s_p[w][k] = a[k];
+    __syncthreads();
+    if (threadIdx.x < RTG_LOSS_EXP_TERMS) {
+        double t = 0.0;
+        for (int k = 0; k < 8; k++) t += s_p[k][threadIdx.x];
+        ws->partial[blockIdx.x][threadIdx.x] = t;
+    }
+}
+
+// One block: warp k adds term k over the blocks' partial sums (fixed lane stride, fixed butterfly); thread 0 writes the
+// statistics loss_grad's scales are made of, the loss parts and dL/d(a, b).
+__global__ void __launch_bounds__(32 * RTG_LOSS_EXP_TERMS) loss_exposure_final_kernel(int nb, float color_weight, float depth_weight,
+                                                                                      LossExposureWs *ws,
+                                                                                      float *__restrict__ dL_dexposure,
+                                                                                      float *__restrict__ loss_out) {
+    __shared__ double s_t[RTG_LOSS_EXP_TERMS];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    double acc = 0.0;
+    for (int k = lane; k < nb; k += 32) acc += ws->partial[k][w];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (lane == 0) s_t[w] = acc;
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+#pragma unroll
+    for (int k = 0; k < 4; k++) ws->st.v[k] = s_t[k];
+    const double nc = s_t[1], nd = s_t[3];
+    const double cl = nc > 0.0 ? s_t[0] / (3.0 * nc) : 0.0, dl = nd > 0.0 ? s_t[2] / nd : 0.0;
+    loss_out[0] = (float)((double)color_weight * cl + (double)depth_weight * dl);
+    loss_out[1] = (float)cl;
+    loss_out[2] = (float)dl;
+    loss_out[3] = (float)nd;
+    const double gcs = nc > 0.0 ? (double)color_weight / (3.0 * nc) : 0.0;
+    dL_dexposure[0] = (float)(gcs * s_t[4]);
+    dL_dexposure[1] = (float)(gcs * s_t[5]);
+}
+
+__global__ void __launch_bounds__(256) loss_exposure_grad_kernel(const float *__restrict__ render, const float *__restrict__ depth,
+                                                                 const int *__restrict__ depth_index, const float *__restrict__ gt_color,
+                                                                 const float *__restrict__ gt_depth, const uint8_t *__restrict__ mask,
+                                                                 int N, int channels_last, float depth_error_max, float color_weight,
+                                                                 float depth_weight, const float *__restrict__ exposure,
+                                                                 const LossExposureWs *ws, float *__restrict__ dL_dcolor,
+                                                                 float *__restrict__ dL_ddepth) {
+    const double nc = ws->st.v[1], nd = ws->st.v[3];
+    const float ea = expf(exposure[0]), eb = exposure[1];
+    // the scale of rtg_loss_l1 times e^a (e^0 = 1 leaves it bit-equal)
+    const float gcs = (nc > 0.0 ? (float)((double)color_weight / (3.0 * nc)) : 0.f) * ea;
+    const float gds = nd > 0.0 ? (float)((double)depth_weight / nd) : 0.f;
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < N; p += gridDim.x * blockDim.x) {
+        const bool m = mask ? (mask[p] != 0) : true;
+        float g0 = 0.f, g1 = 0.f, g2 = 0.f, gd_ = 0.f;
+        if (m) {
+            const float t0 = channels_last ? gt_color[3 * (size_t)p + 0] : gt_color[p];
+            const float t1 = channels_last ? gt_color[3 * (size_t)p + 1] : gt_color[(size_t)N + p];
+            const float t2 = channels_last ? gt_color[3 * (size_t)p + 2] : gt_color[2 * (size_t)N + p];
+            g0 = gcs * sgn(fmaf(ea, render[p], eb) - t0);
+            g1 = gcs * sgn(fmaf(ea, render[(size_t)N + p], eb) - t1);
+            g2 = gcs * sgn(fmaf(ea, render[2 * (size_t)N + p], eb) - t2);
+            const float gd = gt_depth[p];
+            const float e = depth[p] - gd;
+            if (depth_index[p] != -1 && gd > 0.f && e < depth_error_max) gd_ = gds * sgn(e);
+        }
+        dL_dcolor[p] = g0; dL_dcolor[(size_t)N + p] = g1; dL_dcolor[2 * (size_t)N + p] = g2;
+        dL_ddepth[p] = gd_;
+    }
+}
+
 // out (3,H,W) = normal[idx] where idx > -1, zeros elsewhere
 __global__ void __launch_bounds__(256) normal_map_kernel(const float *__restrict__ normal, const int *__restrict__ depth_index, int N,
                                                          float *__restrict__ out) {
@@ -246,6 +361,24 @@ void launch_loss_l1(const float *render, const float *depth, const int *depth_in
     loss_reduce_kernel<<<nb, 256, 0, s>>>(render, depth, depth_index, gt_color, gt_depth, mask, N, channels_last, depth_error_max, st);
     loss_grad_kernel<<<nb, 256, 0, s>>>(render, depth, depth_index, gt_color, gt_depth, mask, N, channels_last, depth_error_max,
                                         color_weight, depth_weight, st, dL_dcolor, dL_ddepth, loss_out);
+}
+
+size_t loss_exposure_ws_bytes() { return sizeof(LossExposureWs); }
+
+void launch_loss_l1_exposure(const float *render, const float *depth, const int *depth_index, const float *gt_color,
+                             const float *gt_depth, const uint8_t *mask, int H, int W, int channels_last, float color_weight,
+                             float depth_weight, float depth_error_max, const float *exposure, float *dL_dcolor, float *dL_ddepth,
+                             float *dL_dexposure, float *loss_out, void *ws, cudaStream_t s) {
+    ProfScope ps(K_ICP_MISC, s);
+    LossExposureWs *w = reinterpret_cast<LossExposureWs *>(ws);
+    const int N = H * W;
+    int nb = (N + 255) / 256;
+    if (nb > RTG_NUM_SMS * 8) nb = RTG_NUM_SMS * 8;
+    loss_exposure_reduce_kernel<<<nb, 256, 0, s>>>(render, depth, depth_index, gt_color, gt_depth, mask, N, channels_last,
+                                                   depth_error_max, exposure, w);
+    loss_exposure_final_kernel<<<1, 32 * RTG_LOSS_EXP_TERMS, 0, s>>>(nb, color_weight, depth_weight, w, dL_dexposure, loss_out);
+    loss_exposure_grad_kernel<<<nb, 256, 0, s>>>(render, depth, depth_index, gt_color, gt_depth, mask, N, channels_last,
+                                                 depth_error_max, color_weight, depth_weight, exposure, w, dL_dcolor, dL_ddepth);
 }
 
 void launch_normal_map(const float *normal, const int *depth_index, int H, int W, float *out, cudaStream_t s) {

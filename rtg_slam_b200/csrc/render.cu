@@ -766,13 +766,18 @@ __global__ void BWD_BOUNDS render_bwd_kernel(const ViewParams vp, const GeomStat
 //                  (a colour channel, or the depth) gets the weight w = 1 for |r| <= delta, delta / |r| otherwise, in
 //                  float from the float residual; the rows hold (w J_a) J_c and (w J_a) r, and the two residual-square
 //                  terms hold sum 2 rho(r) (= sum r^2 while no |r| exceeds delta), so pose_gn_step_kernel is reused as is.
-enum { TAN_IMAGES = 0, TAN_NORMAL_EQ = 1, TAN_NORMAL_EQ_ROBUST = 2 };
+//   TAN_NORMAL_EQ_EXPOSURE[_ROBUST]: the frame's exposure (a, b) estimated with the pose: the colour residual is
+//                  r = e^a C + b - C^ and its Jacobian row (e^a dC/dxi, e^a C, 1), eight columns; the depth rows keep six.
+//                  RTG_GN_EXP_ALL terms per tile, reduced the same way; (e^a, b) is read from the device once per CTA.
+enum { TAN_IMAGES = 0, TAN_NORMAL_EQ = 1, TAN_NORMAL_EQ_ROBUST = 2, TAN_NORMAL_EQ_EXPOSURE = 3, TAN_NORMAL_EQ_EXPOSURE_ROBUST = 4 };
+constexpr bool tan_exposure(const int mode) { return mode == TAN_NORMAL_EQ_EXPOSURE || mode == TAN_NORMAL_EQ_EXPOSURE_ROBUST; }
+constexpr bool tan_robust(const int mode) { return mode == TAN_NORMAL_EQ_ROBUST || mode == TAN_NORMAL_EQ_EXPOSURE_ROBUST; }
 struct GnInputs {
     const float *render, *depth, *gt_color, *gt_depth;
     const uint8_t *mask;
     int channels_last;
     float depth_error_max;
-    double *partial;  // [tiles][RTG_GN_ALL]
+    double *partial;  // [tiles][RTG_GN_ALL], or [tiles][RTG_GN_EXP_ALL] with exposure
 };
 
 // 2 rho(r) of the Huber loss: r^2 inside the threshold, delta (2 |r| - delta) outside
@@ -785,17 +790,21 @@ __device__ __forceinline__ float huber_weight(const float r, const float delta) 
     return a <= delta ? 1.f : delta / a;
 }
 
-// The body of both kernel signatures below; `huber` (colour, depth thresholds) is read by TAN_NORMAL_EQ_ROBUST only.
+// The body of the kernel signatures below; `huber` (colour, depth thresholds) is read by the robust modes only and `ab`
+// (the device exposure) by the exposure modes only.
 template <int MODE>
 __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
                                                     const int *__restrict__ counters, const int *__restrict__ hit_image,
                                                     const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs &in,
-                                                    const float2 huber) {
+                                                    const float2 huber, const double *__restrict__ ab) {
+    constexpr bool EXPOSURE = tan_exposure(MODE);
+    constexpr int NT = EXPOSURE ? RTG_GN_EXP_ALL : RTG_GN_ALL;
     __shared__ float4 s_s0[BATCH], s_s1[BATCH], s_rgb[BATCH];
     __shared__ int s_id[BATCH];
     __shared__ uint32_t s_mask[BATCH];
     __shared__ uint32_t s_max[8];
-    __shared__ double s_red[MODE != TAN_IMAGES ? 8 : 1][RTG_GN_ALL];
+    __shared__ double s_red[MODE != TAN_IMAGES ? 8 : 1][NT];
+    __shared__ float2 s_exp;  // (e^a, b)
 
     const int tile = (int)b.active[blockIdx.x];
     int px, py;
@@ -810,6 +819,8 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(FULL, wmax, o));
     if (lane == 0) s_max[w] = wmax;
+    if constexpr (EXPOSURE)
+        if (threadIdx.x == 0) s_exp = make_float2((float)exp(ab[0]), (float)ab[1]);
     __syncthreads();
     uint32_t m = 0;
 #pragma unroll
@@ -910,17 +921,68 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
     } else {
         const int N = vp.H * vp.W;
         float rc[3] = {0.f, 0.f, 0.f}, rd = 0.f;
+        [[maybe_unused]] float eC[3] = {0.f, 0.f, 0.f};  // e^a C, the colour row's exposure-gain column
         bool sc = inside && (in.mask == nullptr || in.mask[pix] != 0), sd = false;
         if (sc) {
 #pragma unroll
             for (int ch = 0; ch < 3; ch++) {
                 const float gt = in.channels_last ? in.gt_color[3 * (size_t)pix + ch] : in.gt_color[(size_t)ch * N + pix];
-                rc[ch] = in.render[(size_t)ch * N + pix] - gt;
+                if constexpr (EXPOSURE) {
+                    eC[ch] = s_exp.x * in.render[(size_t)ch * N + pix];
+                    rc[ch] = (eC[ch] + s_exp.y) - gt;
+                } else {
+                    rc[ch] = in.render[(size_t)ch * N + pix] - gt;
+                }
             }
             const float gd = in.gt_depth[pix];
             rd = in.depth[pix] - gd;
             sd = hit_image[pix] != -1 && gd > 0.f && rd < in.depth_error_max;  // rtg_loss_l1's depth pixels (signed error)
         }
+        if constexpr (EXPOSURE) {
+            // Each term is reduced as soon as it is formed (double warp butterfly, lane 0 stores the warp's sum), the depth
+            // set first: its tangents are then dead while the 46 colour terms are formed. The __syncwarp orders the
+            // store before the next term; without it ptxas holds the lane-0 sums back and spills.
+            auto put = [&](const int t, const float val) {
+                double x = (double)val;
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(FULL, x, o);
+                if (lane == 0) s_red[w][t] = x;
+                __syncwarp();
+            };
+            constexpr bool ROBUST = tan_robust(MODE);
+            int q = RTG_GN_EXP_COLOR;
+            {
+                const float wd = ROBUST ? huber_weight(rd, huber.y) : 1.f;
+#pragma unroll
+                for (int a = 0; a < 6; a++) {
+                    const float jd = wd * dD[a];
+#pragma unroll
+                    for (int c = a; c < 6; c++, q++) put(q, sd ? jd * dD[c] : 0.f);
+                    put(RTG_GN_EXP_COLOR + 21 + a, sd ? jd * rd : 0.f);
+                }
+                if constexpr (ROBUST) put(RTG_GN_EXP_COLOR + 27, sd ? huber2(rd, huber.y) : 0.f);
+                else put(RTG_GN_EXP_COLOR + 27, sd ? rd * rd : 0.f);
+                put(RTG_GN_EXP_COLOR + 28, sd ? 1.f : 0.f);
+            }
+            const float ea = s_exp.x;
+#pragma unroll
+            for (int k = 0; k < 6; k++) { dC[0][k] *= ea; dC[1][k] *= ea; dC[2][k] *= ea; }
+            // column k of channel ch's Jacobian row (e^a dC/dxi, e^a C, 1)
+            auto jc = [&](const int ch, const int k) { return k < 6 ? dC[ch][k] : (k == 6 ? eC[ch] : 1.f); };
+            const float w0 = ROBUST ? huber_weight(rc[0], huber.x) : 1.f, w1 = ROBUST ? huber_weight(rc[1], huber.x) : 1.f;
+            const float w2 = ROBUST ? huber_weight(rc[2], huber.x) : 1.f;
+            q = 0;
+#pragma unroll
+            for (int a = 0; a < 8; a++) {
+                const float ja0 = w0 * jc(0, a), ja1 = w1 * jc(1, a), ja2 = w2 * jc(2, a);
+#pragma unroll
+                for (int c = a; c < 8; c++, q++) put(q, sc ? ja0 * jc(0, c) + ja1 * jc(1, c) + ja2 * jc(2, c) : 0.f);
+                put(36 + a, sc ? ja0 * rc[0] + ja1 * rc[1] + ja2 * rc[2] : 0.f);
+            }
+            if constexpr (ROBUST) put(44, sc ? huber2(rc[0], huber.x) + huber2(rc[1], huber.x) + huber2(rc[2], huber.x) : 0.f);
+            else put(44, sc ? rc[0] * rc[0] + rc[1] * rc[1] + rc[2] * rc[2] : 0.f);
+            put(45, sc ? 1.f : 0.f);
+        } else {
         float v[RTG_GN_ALL];
         int q = 0;
         if constexpr (MODE == TAN_NORMAL_EQ) {
@@ -965,24 +1027,25 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
             for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(FULL, x, o);
             if (lane == 0) s_red[w][t] = x;
         }
+        }
         __syncthreads();
-        if (threadIdx.x < RTG_GN_ALL) {
+        if (threadIdx.x < NT) {
             double acc = 0.0;
 #pragma unroll
             for (int k = 0; k < 8; k++) acc += s_red[k][threadIdx.x];
-            in.partial[(size_t)tile * RTG_GN_ALL + threadIdx.x] = acc;
+            in.partial[(size_t)tile * NT + threadIdx.x] = acc;
         }
     }
 }
 
-// Two signatures, so that TAN_IMAGES and TAN_NORMAL_EQ keep their parameter list (and their code) and only the robust
-// instantiation carries the Huber thresholds.
+// Three signatures, so that TAN_IMAGES and TAN_NORMAL_EQ keep their parameter list (and their code), only the robust
+// instantiation carries the Huber thresholds and only the exposure ones the pointer to the device exposure.
 template <int MODE>
 __global__ void __launch_bounds__(256) render_tangent_kernel(const ViewParams vp, const GeomState g, const BinState b, const ImgState img,
                                                              const int *__restrict__ counters, const int *__restrict__ hit_image,
                                                              const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs in) {
-    static_assert(MODE != TAN_NORMAL_EQ_ROBUST, "the robust rows take the Huber thresholds");
-    render_tangent_body<MODE>(vp, g, b, img, counters, hit_image, tan, J, in, make_float2(0.f, 0.f));
+    static_assert(MODE == TAN_IMAGES || MODE == TAN_NORMAL_EQ, "the robust rows take the Huber thresholds");
+    render_tangent_body<MODE>(vp, g, b, img, counters, hit_image, tan, J, in, make_float2(0.f, 0.f), nullptr);
 }
 template <int MODE>
 __global__ void __launch_bounds__(256) render_tangent_kernel(const ViewParams vp, const GeomState g, const BinState b, const ImgState img,
@@ -990,7 +1053,15 @@ __global__ void __launch_bounds__(256) render_tangent_kernel(const ViewParams vp
                                                              const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs in,
                                                              const float2 huber) {
     static_assert(MODE == TAN_NORMAL_EQ_ROBUST, "only the robust rows take the Huber thresholds");
-    render_tangent_body<MODE>(vp, g, b, img, counters, hit_image, tan, J, in, huber);
+    render_tangent_body<MODE>(vp, g, b, img, counters, hit_image, tan, J, in, huber, nullptr);
+}
+template <int MODE>
+__global__ void __launch_bounds__(256, 2) render_tangent_kernel(const ViewParams vp, const GeomState g, const BinState b, const ImgState img,
+                                                             const int *__restrict__ counters, const int *__restrict__ hit_image,
+                                                             const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs in,
+                                                             const float2 huber, const double *__restrict__ ab) {
+    static_assert(tan_exposure(MODE), "only the exposure rows read the device exposure");
+    render_tangent_body<MODE>(vp, g, b, img, counters, hit_image, tan, J, in, huber, ab);
 }
 
 // One block: the fixed-order sum of the tiles' rows (one warp per term, fixed lane stride, fixed butterfly), then on one
@@ -1045,6 +1116,89 @@ __global__ void __launch_bounds__(256) pose_gn_step_kernel(const int tiles, cons
     r[7] = (double)status;
 }
 
+// pose_gn_step_kernel for the eight unknowns (rho, phi, a, b). The 8x8 system holds the depth block in its leading 6x6.
+// Damping: the pose diagonals get damping * trace(H[0:6, 0:6]) as above, so that without the exposure columns the pose
+// step is pose_gn_step_kernel's; the exposure diagonals are scaled by (1 + damping) instead, because the pose trace, of
+// order (focal length * image gradient)^2, is many orders above H_bb = color_weight and would freeze (a, b). With no
+// colour term (N_c = 0 or color_weight = 0) the exposure columns are empty: the 6x6 pose system is solved alone and
+// (a, b) is kept. A singular system, an empty selection or an overflowed forward leaves pose and exposure unchanged.
+__global__ void __launch_bounds__(256) pose_gn_exposure_step_kernel(const int tiles, const double *__restrict__ partial,
+                                                                     const int *__restrict__ counters, const RtgPoseGN s,
+                                                                     double *__restrict__ ab) {
+    __shared__ double s_tot[RTG_GN_EXP_ALL];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int term = w; term < RTG_GN_EXP_ALL; term += 8) {
+        double acc = 0.0;
+        for (int t = lane; t < tiles; t += 32) acc += partial[(size_t)t * RTG_GN_EXP_ALL + term];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL, acc, o);
+        if (lane == 0) s_tot[term] = acc;
+    }
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    const double *cs = s_tot, *ds = s_tot + RTG_GN_EXP_COLOR;
+    const double nc = 3.0 * cs[45], nd = ds[28];
+    const double wc = nc > 0.0 ? (double)s.color_weight / nc : 0.0, wd = nd > 0.0 ? (double)s.depth_weight / nd : 0.0;
+    double A[8][8], bvec[8], x[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    int q = 0;
+#pragma unroll
+    for (int a = 0; a < 8; a++) {
+#pragma unroll
+        for (int c = a; c < 8; c++, q++) { const double v = wc * cs[q]; A[a][c] = v; A[c][a] = v; }
+        bvec[a] = -(wc * cs[36 + a]);
+    }
+    q = 0;
+#pragma unroll
+    for (int a = 0; a < 6; a++) {
+#pragma unroll
+        for (int c = a; c < 6; c++, q++) { const double v = A[a][c] + wd * ds[q]; A[a][c] = v; A[c][a] = v; }
+        bvec[a] -= wd * ds[21 + a];
+    }
+    double trace = 0.0;
+#pragma unroll
+    for (int a = 0; a < 6; a++) trace += A[a][a];
+#pragma unroll
+    for (int a = 0; a < 6; a++) A[a][a] += trace * (double)s.damping;
+    A[6][6] *= 1.0 + (double)s.damping;
+    A[7][7] *= 1.0 + (double)s.damping;
+    const bool exposed = wc > 0.0;
+    int status = RTG_POSE_GN_OK;
+    if (counters[2] != 0) status = RTG_POSE_GN_OVERFLOW;
+    else if (nc + nd == 0.0) status = RTG_POSE_GN_EMPTY;
+    else if (exposed) {
+        if (!solve_n<8>(A, bvec, x)) status = RTG_POSE_GN_SINGULAR;
+    } else {
+        double A6[6][6];
+#pragma unroll
+        for (int a = 0; a < 6; a++)
+#pragma unroll
+            for (int c = 0; c < 6; c++) A6[a][c] = A[a][c];
+        if (!solve6(A6, bvec, x)) status = RTG_POSE_GN_SINGULAR;
+    }
+    if (status == RTG_POSE_GN_OK) {
+        double Tm[4][4], E[3][4];
+#pragma unroll
+        for (int i = 0; i < 16; i++) Tm[i / 4][i % 4] = s.pose[i];
+        se3_exp_twist(x, E);
+        pose_left_update(E, Tm, s.pose, s.projection, s.viewmatrix, s.projmatrix, s.campos);
+        if (exposed) { ab[0] += x[6]; ab[1] += x[7]; }
+    } else {
+#pragma unroll
+        for (int a = 0; a < 6; a++) x[a] = 0.0;
+    }
+    const double ec = 0.5 * wc * cs[44], ed = 0.5 * wd * ds[27];
+    double *r = s.report;
+    r[0] = ec + ed; r[1] = ec; r[2] = ed; r[3] = nc; r[4] = nd;
+    r[5] = sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
+    r[6] = sqrt(x[3] * x[3] + x[4] * x[4] + x[5] * x[5]);
+    r[7] = (double)status;
+}
+
+size_t pose_gn_exposure_scratch_bytes(int P, int H, int W) {
+    const size_t tiles = (size_t)((W + RTG_TILE - 1) / RTG_TILE) * ((H + RTG_TILE - 1) / RTG_TILE);
+    return align_up((size_t)(P > 0 ? P : 0) * RTG_TAN_ROW * sizeof(float4), 256) + tiles * RTG_GN_EXP_ALL * sizeof(double);
+}
+
 size_t pose_gn_scratch_bytes(int P, int H, int W) {
     const size_t tiles = (size_t)((W + RTG_TILE - 1) / RTG_TILE) * ((H + RTG_TILE - 1) / RTG_TILE);
     return align_up((size_t)(P > 0 ? P : 0) * RTG_TAN_ROW * sizeof(float4), 256) + tiles * RTG_GN_ALL * sizeof(double);
@@ -1071,6 +1225,22 @@ void launch_pose_gn_normal_eq_step(const ViewParams &vp, int P, const GeomState 
     else
         render_tangent_kernel<TAN_NORMAL_EQ><<<T, 256, 0, s>>>(vp, g, b, img, counters, st.hit_depth, tan_rows(st.scratch), nullptr, in);
     pose_gn_step_kernel<<<1, 256, 0, s>>>(T, in.partial, counters, st);
+}
+
+void launch_pose_gn_exposure_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                  const int32_t *counters, const RtgPoseGN &st, const RtgPoseRobust &robust, double *ab,
+                                  cudaStream_t s) {
+    const int T = vp.tiles_x * vp.tiles_y;
+    GnInputs in{st.render, st.depth, st.gt_color, st.gt_depth, st.render_mask, st.gt_channels_last, st.depth_error_max,
+                gn_partial(st.scratch, P)};
+    const float2 huber = make_float2(robust.color_delta, robust.depth_delta);
+    if (robust.kernel == RTG_ROBUST_HUBER)
+        render_tangent_kernel<TAN_NORMAL_EQ_EXPOSURE_ROBUST><<<T, 256, 0, s>>>(vp, g, b, img, counters, st.hit_depth,
+                                                                              tan_rows(st.scratch), nullptr, in, huber, ab);
+    else
+        render_tangent_kernel<TAN_NORMAL_EQ_EXPOSURE><<<T, 256, 0, s>>>(vp, g, b, img, counters, st.hit_depth, tan_rows(st.scratch),
+                                                                       nullptr, in, huber, ab);
+    pose_gn_exposure_step_kernel<<<1, 256, 0, s>>>(T, in.partial, counters, st, ab);
 }
 
 void launch_render_fwd(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img, const int32_t *counters,

@@ -27,32 +27,40 @@ def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def _l1_inputs(render, depth, depth_index, gt_color, gt_depth, render_mask):
+    """The checked, contiguous inputs of both L1 entries: (render, depth, depth_index, gt_color, gt_depth, mask, H, W,
+    channels_last)."""
+    for name, t in (("render", render), ("depth", depth), ("gt_color", gt_color), ("gt_depth", gt_depth)):
+        if not t.is_cuda or t.dtype != torch.float32:
+            raise TypeError(f"{name} must be a CUDA float32 tensor")
+    if depth_index.dtype != torch.int32:
+        raise TypeError("depth_index must be int32 (the rasterizer's depth_index_map)")
+    _, H, W = render.shape
+    render, depth, depth_index = render.contiguous(), depth.contiguous(), depth_index.contiguous()
+    gt_color, gt_depth = gt_color.contiguous(), gt_depth.contiguous()
+    if gt_color.shape == (H, W, 3):
+        channels_last = 1
+    elif gt_color.shape == (3, H, W):
+        channels_last = 0
+    else:
+        raise ValueError("gt_color must be (H,W,3) or (3,H,W)")
+    if gt_depth.numel() != H * W:
+        raise ValueError("gt_depth must have H*W elements")
+    mask = None
+    if render_mask is not None:
+        mask = render_mask.to(torch.uint8).contiguous() if render_mask.dtype != torch.uint8 else render_mask.contiguous()
+        if mask.numel() != H * W:
+            raise ValueError("render_mask must have H*W elements")
+    return render, depth, depth_index, gt_color, gt_depth, mask, H, W, channels_last
+
+
 class _FusedL1(torch.autograd.Function):
     @staticmethod
     def forward(ctx, render, depth, depth_index, gt_color, gt_depth, render_mask, color_weight, depth_weight, depth_error_max):
         L = _lib.lib()
         dev = render.device
-        for name, t in (("render", render), ("depth", depth), ("gt_color", gt_color), ("gt_depth", gt_depth)):
-            if not t.is_cuda or t.dtype != torch.float32:
-                raise TypeError(f"{name} must be a CUDA float32 tensor")
-        if depth_index.dtype != torch.int32:
-            raise TypeError("depth_index must be int32 (the rasterizer's depth_index_map)")
-        _, H, W = render.shape
-        render, depth, depth_index = render.contiguous(), depth.contiguous(), depth_index.contiguous()
-        gt_color, gt_depth = gt_color.contiguous(), gt_depth.contiguous()
-        if gt_color.shape == (H, W, 3):
-            channels_last = 1
-        elif gt_color.shape == (3, H, W):
-            channels_last = 0
-        else:
-            raise ValueError("gt_color must be (H,W,3) or (3,H,W)")
-        if gt_depth.numel() != H * W:
-            raise ValueError("gt_depth must have H*W elements")
-        mask = None
-        if render_mask is not None:
-            mask = render_mask.to(torch.uint8).contiguous() if render_mask.dtype != torch.uint8 else render_mask.contiguous()
-            if mask.numel() != H * W:
-                raise ValueError("render_mask must have H*W elements")
+        render, depth, depth_index, gt_color, gt_depth, mask, H, W, channels_last = _l1_inputs(render, depth, depth_index, gt_color,
+                                                                                               gt_depth, render_mask)
         g_color = torch.empty_like(render)
         g_depth = torch.empty_like(depth)
         out = torch.empty(4, dtype=torch.float32, device=dev)
@@ -69,10 +77,53 @@ class _FusedL1(torch.autograd.Function):
         return g_color * grad_loss, g_depth * grad_loss, None, None, None, None, None, None, None
 
 
+_EXPOSURE_WS = {}
+
+
+class _FusedL1Exposure(torch.autograd.Function):
+    """_FusedL1 of a render seen under the frame exposure (a, b): rtg_loss_l1_exposure, which also returns dL/d(a, b)."""
+
+    @staticmethod
+    def forward(ctx, render, depth, depth_index, gt_color, gt_depth, render_mask, color_weight, depth_weight, depth_error_max,
+                exposure):
+        L = _lib.lib()
+        dev = render.device
+        render, depth, depth_index, gt_color, gt_depth, mask, H, W, channels_last = _l1_inputs(render, depth, depth_index, gt_color,
+                                                                                               gt_depth, render_mask)
+        if not exposure.is_cuda or exposure.dtype != torch.float32 or exposure.shape != (2,):
+            raise TypeError("exposure must be a (2,) CUDA float32 tensor")
+        exposure = exposure.contiguous()
+        idx = dev.index if dev.index is not None else torch.cuda.current_device()
+        if idx not in _EXPOSURE_WS:
+            _EXPOSURE_WS[idx] = torch.zeros(L.rtg_loss_l1_exposure_workspace_bytes(), dtype=torch.uint8, device=torch.device("cuda", idx))
+        g_color = torch.empty_like(render)
+        g_depth = torch.empty_like(depth)
+        g_exposure = torch.empty(2, dtype=torch.float32, device=dev)
+        out = torch.empty(4, dtype=torch.float32, device=dev)
+        check(L.rtg_loss_l1_exposure(_p(render), _p(depth), _p(depth_index), _p(gt_color), _p(gt_depth), _p(mask), H, W, channels_last,
+                                     float(color_weight), float(depth_weight), float(depth_error_max), _p(exposure), _p(g_color),
+                                     _p(g_depth), _p(g_exposure), _p(out), _p(_EXPOSURE_WS[idx]),
+                                     C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "rtg_loss_l1_exposure")
+        ctx.save_for_backward(g_color, g_depth, g_exposure)
+        ctx.mark_non_differentiable(out)
+        return out[0], out
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_parts):
+        g_color, g_depth, g_exposure = ctx.saved_tensors
+        return g_color * grad_loss, g_depth * grad_loss, None, None, None, None, None, None, None, g_exposure * grad_loss
+
+
 def l1_color_depth_loss(render_output, gt_color, gt_depth, render_mask=None, color_weight=0.8, depth_weight=1.0,
-                        depth_error_max=0.1):
+                        depth_error_max=0.1, exposure=None):
     """`render_output` is the dict of Renderer.render. Defaults: color_weight / depth_weight / add_depth_thres of
-    configs/base.yaml:76-77,51. Returns (loss, parts) with parts = tensor [loss, colour_l1, depth_l1, n_depth]."""
+    configs/base.yaml:76-77,51. Returns (loss, parts) with parts = tensor [loss, colour_l1, depth_l1, n_depth].
+    `exposure`: None, or a (2,) CUDA float32 tensor (a, b): the colour residual becomes e^a render + b - gt_color
+    (rtg_loss_l1_exposure) and the loss is differentiable with respect to the render and to `exposure`, so that a keyframe
+    can be fitted under its camera's brightness without baking it into the map."""
+    if exposure is not None:
+        return _FusedL1Exposure.apply(render_output["render"], render_output["depth"], render_output["depth_index_map"], gt_color,
+                                      gt_depth, render_mask, color_weight, depth_weight, depth_error_max, exposure)
     return _FusedL1.apply(render_output["render"], render_output["depth"], render_output["depth_index_map"], gt_color, gt_depth,
                           render_mask, color_weight, depth_weight, depth_error_max)
 

@@ -24,6 +24,11 @@ twist directions, forms and solves the 6x6 normal equations and updates the pose
 returns those tangent images themselves. Optionally it runs coarse to fine over an image pyramid (`downsample_frame`,
 `level_camera`) and weighs each residual by the Huber loss (rtg_splat_pose_gn_step_robust).
 
+Both refiners can estimate the frame's exposure with the pose (`exposure=`): the camera's pixel values are modelled as
+e^a C + b of the map's radiance C, one gain and one offset per frame (`apply_exposure`), so that auto-exposure is not
+explained by a pose change. `refine_gn` then solves for eight unknowns per step (rtg_splat_pose_gn_step_exposure); `refine`
+takes the loss under the exposure (rtg_loss_l1_exposure) and one more Adam step on (a, b).
+
 When to track with either (every frame, after ICP, on keyframes only) is SLAM policy and is left to the caller."""
 from __future__ import annotations
 
@@ -36,6 +41,7 @@ import torch
 from . import _lib, rasterizer
 from ._lib import RtgPoseAdam, RtgPoseGN, check
 from .loss import l1_color_depth_loss
+from .optim import FusedAdam
 from .rasterizer import CapacityOverflow, GaussianRasterizationSettings, _forward_native, _make_view, rasterize_gaussians
 from .render import Renderer
 
@@ -77,6 +83,23 @@ def pose_jacobian(raster_settings, means3D, opacities, shs=None, colors_precomp=
                                         C.c_void_p(scratch.data_ptr()), C.c_void_p(J.data_ptr()),
                                         C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "rtg_splat_pose_tangents")
         return outs, J
+
+
+def apply_exposure(image, exposure):
+    """`image` seen under the exposure (a, b): e^a image + b. `exposure`: a pair of floats or a 2-element tensor."""
+    a, b = exposure[0], exposure[1]
+    return (torch.exp(a) if torch.is_tensor(a) else math.exp(a)) * image + b
+
+
+def _exposure_pair(exposure, dev, dtype):
+    """A fresh (2,) tensor (a, b) on `dev` from a pair of floats or a 2-element tensor."""
+    if torch.is_tensor(exposure):
+        t = exposure.detach().to(device=dev, dtype=dtype).reshape(-1).clone()
+    else:
+        t = torch.tensor([float(x) for x in exposure], dtype=dtype, device=dev)
+    if t.numel() != 2:
+        raise ValueError("exposure must hold two numbers (a, b)")
+    return t
 
 
 def level_camera(camera, s):
@@ -181,7 +204,7 @@ class PoseRefiner:
 
     def refine_gn(self, camera, gaussian_data, gt_color, gt_depth, iters, damping=1e-4, color_weight=0.8, depth_weight=1.0,
                   render_mask=None, tile_mask=None, depth_error_max=0.1, scales=(1,), robust=None, color_delta=0.1,
-                  depth_delta=0.05):
+                  depth_delta=0.05, exposure=None):
         """Gauss-Newton refinement of the pose on the squared colour + depth residuals (rtg_splat_pose_gn_step): per
         iteration the rasterizer forward, then the forward-mode tangents of the render along the six twist directions, the
         normal equations over rtg_loss_l1's pixel selection, the damped solve (H + damping * trace(H) * I) and
@@ -197,6 +220,12 @@ class PoseRefiner:
         `robust`: None (squared residuals) or "huber" (rtg_splat_pose_gn_step_robust: Huber loss with thresholds
         `color_delta` in colour units and `depth_delta` in map units, minimised by reweighted least squares).
         The defaults (one level, no robust loss) run one rtg_splat_pose_gn_step per iteration and nothing else.
+        `exposure`: None, or the starting exposure (a0, b0) of the frame (a pair of floats or a 2-element tensor; (0, 0)
+        for none, the previous frame's estimate when tracking a sequence). The colour residual becomes e^a C + b - C^ and
+        each step solves for (rho, phi, a, b) (rtg_splat_pose_gn_step_exposure: the pose diagonals damped as above, the
+        exposure diagonals scaled by 1 + damping), with any `scales` and `robust`. A block mean is linear, so (a, b) of the
+        frame is (a, b) of every level and carries over as the pose does. A third value is then returned: the estimate,
+        a (2,) float64 CUDA tensor.
 
         Returns (W2C, report): the refined pose, a (4, 4) float64 CUDA tensor, and the finest level's last step's report,
         a float64 CUDA tensor [E, E_colour, E_depth, N_c, N_d, |rho|, |phi|, status] (E evaluated before that step; status
@@ -232,7 +261,8 @@ class PoseRefiner:
                 raise ValueError("render_mask must have H*W elements")
         P = int(g["xyz"].shape[0])
         L = _lib.lib()
-        scratch = torch.empty((int(L.rtg_splat_pose_gn_scratch_bytes(P, H, W)),), dtype=torch.uint8, device=dev)  # the finest level's
+        scratch_bytes = L.rtg_splat_pose_gn_scratch_bytes if exposure is None else L.rtg_splat_pose_gn_exposure_scratch_bytes
+        scratch = torch.empty((int(scratch_bytes(P, H, W)),), dtype=torch.uint8, device=dev)  # the finest level's
         report = torch.zeros(_lib.RTG_POSE_GN_REPORT_LEN, dtype=torch.float64, device=dev)
 
         def state(projection, gt_color, gt_depth, mask, channels_last):
@@ -256,11 +286,17 @@ class PoseRefiner:
             lproj = cam.projection_matrix.to(device=dev, dtype=torch.float32).contiguous()
             targets = downsample_frame(gt_color, gt_depth.view(H, W), sc, mask, tile_mask)
             levels.append((self._settings(cam, dev, view, proj, campos), lproj, state(lproj, *targets[:3], 0), targets[3], targets))
-        if robust is None:
+        r = _lib.RtgPoseRobust()
+        if robust is not None:
+            r.kernel, r.color_delta, r.depth_delta = _lib.RTG_ROBUST_HUBER, float(color_delta), float(depth_delta)
+        if exposure is not None:
+            ab = _exposure_pair(exposure, dev, torch.float64)
+            ex = _lib.RtgPoseExposure()
+            ex.ab = ab.data_ptr()
+            step, extra = L.rtg_splat_pose_gn_step_exposure, (C.byref(r), C.byref(ex))
+        elif robust is None:
             step, extra = L.rtg_splat_pose_gn_step, ()
         else:
-            r = _lib.RtgPoseRobust()
-            r.kernel, r.color_delta, r.depth_delta = _lib.RTG_ROBUST_HUBER, float(color_delta), float(depth_delta)
             step, extra = L.rtg_splat_pose_gn_step_robust, (C.byref(r),)
         st = rasterizer._state(dev)
         for (lrs, lproj, s, ltm, _), n in zip(levels, level_iters):
@@ -278,16 +314,20 @@ class PoseRefiner:
                 s.render, s.depth, s.hit_depth = outs[0].data_ptr(), outs[1].data_ptr(), outs[3].data_ptr()
                 check(step(*_native_args(lrs, saved, ins, dev), C.byref(s), *extra,
                            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), step.__name__)
-        return pose, report
+        return (pose, report) if exposure is None else (pose, report, ab)
 
     def refine(self, camera, gaussian_data, gt_color, gt_depth, iters, lr_rot, lr_trans, color_weight=0.8, depth_weight=1.0,
-               render_mask=None, tile_mask=None):
+               render_mask=None, tile_mask=None, exposure=None, lr_exposure=0.01):
         """`camera`: a reference-Camera-like object (world_view_transform, projection_matrix, FoVx, FoVy, image_height,
         image_width, cx, cy); its pose is the starting point and is not modified. `gaussian_data`: the dict Renderer.render
         takes (xyz, opacity, shs, scales, rotations); it is not differentiated. gt_color (H,W,3) or (3,H,W), gt_depth
         (H,W); render_mask (H,W) selects the colour / depth pixels of the loss, tile_mask the rendered 16x16 tiles.
         Adam (betas 0.9, 0.999, eps 1e-8) starts from zero moments on every call; lr_rot (radians) and lr_trans (map
         units) are its step sizes.
+        `exposure`: None, or the starting exposure (a0, b0) of the frame as in `refine_gn`. The loss is then taken under
+        it (l1_color_depth_loss(..., exposure=)), and (a, b) takes its own Adam step of size `lr_exposure` per iteration
+        (optim.FusedAdam, one more launch; the pose step is unchanged). A third value is then returned: the estimate, a
+        (2,) float32 CUDA tensor.
 
         Returns (W2C, parts): the refined world-to-camera pose, a (4, 4) float64 CUDA tensor, and the loss parts of the
         last iteration's render, [loss, colour L1, depth L1, n_depth] (l1_color_depth_loss; evaluated before its step)."""
@@ -305,23 +345,32 @@ class PoseRefiner:
         st.beta1, st.beta2, st.eps = 0.9, 0.999, 1e-8
         L = _lib.lib()
         parts = None
+        ab = adam_ab = None
+        if exposure is not None:
+            ab = _exposure_pair(exposure, dev, torch.float32).requires_grad_(True)
+            adam_ab = FusedAdam([ab], lr=float(lr_exposure), betas=(0.9, 0.999), eps=1e-8)
         with torch.enable_grad():
             for it in range(iters):
                 for attempt in range(2):
                     out = rasterize_gaussians(g["xyz"], g["shs"], None, g["opacity"], g["scales"], g["rotations"], None,
                                               tile_mask, rs)
                     loss, parts = l1_color_depth_loss({"render": out[0], "depth": out[1], "depth_index_map": out[3]},
-                                                      gt_color, gt_depth, render_mask, color_weight, depth_weight)
+                                                      gt_color, gt_depth, render_mask, color_weight, depth_weight, exposure=ab)
                     try:
                         loss.backward()
                         break
                     except CapacityOverflow:  # this render was empty; the capacity has been raised: render it again
                         if attempt:
                             raise
+                        if ab is not None:
+                            ab.grad = None  # the empty render's exposure gradient is not this iteration's
                 st.dL_dviewmatrix, st.dL_dprojmatrix, st.dL_dcampos = (
                     t.grad.data_ptr() if t.grad is not None else None for t in (view, proj, campos))
                 st.step = it + 1
                 check(L.rtg_pose_adam_step(C.byref(st), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
                       "rtg_pose_adam_step")
                 view.grad = proj.grad = campos.grad = None
-        return pose, parts
+                if ab is not None:
+                    adam_ab.step()
+                    ab.grad = None
+        return (pose, parts) if exposure is None else (pose, parts, ab.detach())

@@ -524,8 +524,10 @@ int rtg_icp_predict_pose(const RtgIcpLevel *levels, int32_t n_levels, float dist
  *            depth_error_max and the render mask,  loss = color_weight*colour + depth_weight*depth.
  * render (3,H,W), depth (1,H,W), depth_index (1,H,W) are rasterizer outputs; gt_color is (H,W,3) if
  * gt_channels_last else (3,H,W); gt_depth (H,W); render_mask (H,W) bytes. loss_out: 4 device floats
- * {loss, colour, depth, n_depth}. An empty selection contributes 0 (torch's mean of an empty tensor is NaN).
- * ws: rtg_loss_workspace_bytes() bytes. */
+ * {loss, colour, depth, n_depth}. An empty selection contributes 0 (torch's mean of an empty tensor is NaN). The sums are
+ * formed in double from per-block partial sums added in a fixed order (no atomics): identical inputs give bit-identical
+ * outputs. ws: rtg_loss_workspace_bytes() bytes (about 66 KB), 8-byte aligned; one workspace serves all three losses.
+ * Rejects a NULL pointer (render_mask may be NULL), H, W <= 0 and a misaligned ws on the host before any CUDA work. */
 size_t rtg_loss_workspace_bytes(void);
 int rtg_loss_l1(const float *render, const float *depth, const int32_t *depth_index, const float *gt_color, const float *gt_depth,
                 const uint8_t *render_mask, int32_t H, int32_t W, int32_t gt_channels_last, float color_weight, float depth_weight,
@@ -535,10 +537,9 @@ int rtg_loss_l1(const float *render, const float *depth, const int32_t *depth_in
  * term is the mean of |r|, r = e^a render + b - gt_color, over the same pixels; the depth term is unchanged. Written:
  *   dL_dcolor = color_weight / N_c e^a sgn(r),  dL_ddepth as rtg_loss_l1,
  *   dL_dexposure (2 device floats) = color_weight / N_c (sum sgn(r) e^a render, sum sgn(r)),  N_c = 3 x selected pixels,
- * and loss_out as rtg_loss_l1. exposure = (0, 0) gives rtg_loss_l1's loss and gradients. The sums are formed in double from
- * per-block partial sums added in a fixed order (no atomics): identical inputs give bit-identical outputs.
- * ws: rtg_loss_l1_exposure_workspace_bytes() bytes. Rejects a NULL pointer (render_mask may be NULL) and H, W <= 0 on the
- * host before any CUDA work. */
+ * and loss_out as rtg_loss_l1. exposure = (0, 0) gives rtg_loss_l1's loss_out and gradients bit for bit. Sums, workspace and
+ * validation as rtg_loss_l1 (rtg_loss_l1_exposure_workspace_bytes() == rtg_loss_workspace_bytes()); exposure and
+ * dL_dexposure must not be NULL. */
 size_t rtg_loss_l1_exposure_workspace_bytes(void);
 int rtg_loss_l1_exposure(const float *render, const float *depth, const int32_t *depth_index, const float *gt_color,
                          const float *gt_depth, const uint8_t *render_mask, int32_t H, int32_t W, int32_t gt_channels_last,
@@ -550,7 +551,8 @@ int rtg_loss_l1_exposure(const float *render, const float *depth, const int32_t 
  *            gt_normal != 0,  loss = color_weight*colour + depth_weight*depth + normal_weight*normal.
  * render_normal (3,H,W) is Renderer.render's "normal"; gt_normal (H,W,3); dL_dnormal (3,H,W). With normal_weight == 0 the
  * three normal pointers may be NULL. loss_out: 8 device floats {loss, colour, depth, n_depth, normal, n_normal, 0, 0}:
- * everything Mapping.loss_update reports (mapper.py:459-466) in one buffer, one read-back instead of six .item() calls. */
+ * everything Mapping.loss_update reports (mapper.py:459-466) in one buffer, one read-back instead of six .item() calls.
+ * Sums, workspace and validation as rtg_loss_l1. */
 int rtg_loss_mapping(const float *render, const float *depth, const float *render_normal, const int32_t *depth_index,
                      const float *gt_color, const float *gt_depth, const float *gt_normal, const uint8_t *render_mask, int32_t H, int32_t W,
                      int32_t gt_channels_last, float color_weight, float depth_weight, float normal_weight, float depth_error_max,

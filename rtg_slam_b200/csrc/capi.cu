@@ -46,7 +46,6 @@ void launch_loss_mapping(const float *render, const float *depth, const float *r
                          const float *gt_color, const float *gt_depth, const float *gt_normal, const uint8_t *mask, int H, int W,
                          int channels_last, float color_weight, float depth_weight, float normal_weight, float depth_error_max,
                          float *dL_dcolor, float *dL_ddepth, float *dL_dnormal, float *loss_out, void *ws, cudaStream_t s);
-size_t loss_exposure_ws_bytes();
 void launch_loss_l1_exposure(const float *render, const float *depth, const int *depth_index, const float *gt_color,
                              const float *gt_depth, const uint8_t *mask, int H, int W, int channels_last, float color_weight,
                              float depth_weight, float depth_error_max, const float *exposure, float *dL_dcolor, float *dL_ddepth,
@@ -833,30 +832,40 @@ int rtg_icp_fill_model_depth(float *render_depth, const float *frame_depth, cons
     return check_launch("rtg_icp_fill_model_depth");
 }
 
+// The checks shared by the three frame losses; `ws` holds doubles.
+static int validate_loss(const char *who, const float *render, const float *depth, const int32_t *depth_index,
+                         const float *gt_color, const float *gt_depth, int32_t H, int32_t W, const float *dL_dcolor,
+                         const float *dL_ddepth, const float *loss_out, const void *ws) {
+    if (H <= 0 || W <= 0) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": H and W must be >= 1");
+    if (!render || !depth || !depth_index || !gt_color || !gt_depth || !dL_dcolor || !dL_ddepth || !loss_out || !ws)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pointer");
+    if (((uintptr_t)ws) & 7) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": ws must be 8-byte aligned");
+    return RTG_OK;
+}
+
 size_t rtg_loss_workspace_bytes(void) { return rtg::loss_ws_bytes(); }
 
 int rtg_loss_l1(const float *render, const float *depth, const int32_t *depth_index, const float *gt_color, const float *gt_depth,
                 const uint8_t *render_mask, int32_t H, int32_t W, int32_t gt_channels_last, float color_weight, float depth_weight,
                 float depth_error_max, float *dL_dcolor, float *dL_ddepth, float *loss_out, void *ws, void *stream) {
-    if (!render || !depth || !depth_index || !gt_color || !gt_depth || !dL_dcolor || !dL_ddepth || !loss_out || !ws || H <= 0 || W <= 0)
-        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_loss_l1: bad arguments");
+    const char *who = "rtg_loss_l1";
+    int rc = validate_loss(who, render, depth, depth_index, gt_color, gt_depth, H, W, dL_dcolor, dL_ddepth, loss_out, ws);
+    if (rc) return rc;
     rtg::launch_loss_l1(render, depth, depth_index, gt_color, gt_depth, render_mask, H, W, gt_channels_last, color_weight, depth_weight,
                         depth_error_max, dL_dcolor, dL_ddepth, loss_out, ws, reinterpret_cast<cudaStream_t>(stream));
-    return check_launch("rtg_loss_l1");
+    return check_launch(who);
 }
 
-size_t rtg_loss_l1_exposure_workspace_bytes(void) { return rtg::loss_exposure_ws_bytes(); }
+size_t rtg_loss_l1_exposure_workspace_bytes(void) { return rtg::loss_ws_bytes(); }
 
 int rtg_loss_l1_exposure(const float *render, const float *depth, const int32_t *depth_index, const float *gt_color,
                          const float *gt_depth, const uint8_t *render_mask, int32_t H, int32_t W, int32_t gt_channels_last,
                          float color_weight, float depth_weight, float depth_error_max, const float *exposure, float *dL_dcolor,
                          float *dL_ddepth, float *dL_dexposure, float *loss_out, void *ws, void *stream) {
     const char *who = "rtg_loss_l1_exposure";
-    if (H <= 0 || W <= 0) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": H and W must be >= 1");
-    if (!render || !depth || !depth_index || !gt_color || !gt_depth || !dL_dcolor || !dL_ddepth || !loss_out || !ws)
-        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pointer");
+    int rc = validate_loss(who, render, depth, depth_index, gt_color, gt_depth, H, W, dL_dcolor, dL_ddepth, loss_out, ws);
+    if (rc) return rc;
     if (!exposure || !dL_dexposure) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL exposure / dL_dexposure");
-    if (((uintptr_t)ws) & 7) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": ws must be 8-byte aligned");
     rtg::launch_loss_l1_exposure(render, depth, depth_index, gt_color, gt_depth, render_mask, H, W, gt_channels_last, color_weight,
                                  depth_weight, depth_error_max, exposure, dL_dcolor, dL_ddepth, dL_dexposure, loss_out, ws,
                                  reinterpret_cast<cudaStream_t>(stream));
@@ -867,14 +876,15 @@ int rtg_loss_mapping(const float *render, const float *depth, const float *rende
                      const float *gt_color, const float *gt_depth, const float *gt_normal, const uint8_t *render_mask, int32_t H, int32_t W,
                      int32_t gt_channels_last, float color_weight, float depth_weight, float normal_weight, float depth_error_max,
                      float *dL_dcolor, float *dL_ddepth, float *dL_dnormal, float *loss_out, void *ws, void *stream) {
-    if (!render || !depth || !depth_index || !gt_color || !gt_depth || !dL_dcolor || !dL_ddepth || !loss_out || !ws || H <= 0 || W <= 0)
-        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_loss_mapping: bad arguments");
+    const char *who = "rtg_loss_mapping";
+    int rc = validate_loss(who, render, depth, depth_index, gt_color, gt_depth, H, W, dL_dcolor, dL_ddepth, loss_out, ws);
+    if (rc) return rc;
     if (normal_weight > 0.f && (!render_normal || !gt_normal || !dL_dnormal))
-        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_loss_mapping: normal_weight > 0 needs render_normal, gt_normal and dL_dnormal");
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": normal_weight > 0 needs render_normal, gt_normal and dL_dnormal");
     rtg::launch_loss_mapping(render, depth, render_normal, depth_index, gt_color, gt_depth, gt_normal, render_mask, H, W, gt_channels_last,
                              color_weight, depth_weight, normal_weight, depth_error_max, dL_dcolor, dL_ddepth, dL_dnormal, loss_out, ws,
                              reinterpret_cast<cudaStream_t>(stream));
-    return check_launch("rtg_loss_mapping");
+    return check_launch(who);
 }
 
 size_t rtg_ssim_workspace_bytes(int32_t C, int32_t H, int32_t W) {

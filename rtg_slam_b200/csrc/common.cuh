@@ -142,6 +142,18 @@ __device__ __forceinline__ float3 xvec4x3T(const float3 p, const float *m) {
 __device__ __forceinline__ int arg_max3(float a, float b, float c) { return (a >= b && a >= c) ? 0 : ((b >= a && b >= c) ? 1 : 2); }
 __device__ __forceinline__ int arg_min3(float a, float b, float c) { return (a <= b && a <= c) ? 0 : ((b <= a && b <= c) ? 1 : 2); }
 
+// ------------------------------------------------------------------ the frame residual's pixel rules
+// One definition for the L1 / mapping losses (loss.cu) and the Gauss-Newton tracker's residuals (render.cu).
+// Channel c of the measured colour at pixel p of an N-pixel frame: gt_color is (H,W,3) if channels_last else (3,H,W).
+__device__ __forceinline__ float frame_color(const float *gt_color, int channels_last, int N, int p, int c) {
+    return channels_last ? gt_color[3 * (size_t)p + c] : gt_color[(size_t)c * N + p];
+}
+// A depth pixel of the loss: the render hit a Gaussian, the frame measured a depth, and the signed error
+// err = depth - gt_depth is below depth_error_max.
+__device__ __forceinline__ bool frame_depth_pixel(int hit, float gt_depth, float err, float depth_error_max) {
+    return hit != -1 && gt_depth > 0.f && err < depth_error_max;
+}
+
 // Tile rectangle touched by a splat of integer radius r centred at p (same rounding as the
 // reference's getRect, auxiliary.h:49-57).
 __device__ __forceinline__ void tile_rect(const float2 p, int r, int gx, int gy, int &x0, int &y0, int &x1, int &y1) {

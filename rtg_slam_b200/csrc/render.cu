@@ -926,7 +926,7 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
         if (sc) {
 #pragma unroll
             for (int ch = 0; ch < 3; ch++) {
-                const float gt = in.channels_last ? in.gt_color[3 * (size_t)pix + ch] : in.gt_color[(size_t)ch * N + pix];
+                const float gt = frame_color(in.gt_color, in.channels_last, N, pix, ch);
                 if constexpr (EXPOSURE) {
                     eC[ch] = s_exp.x * in.render[(size_t)ch * N + pix];
                     rc[ch] = (eC[ch] + s_exp.y) - gt;
@@ -936,7 +936,7 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
             }
             const float gd = in.gt_depth[pix];
             rd = in.depth[pix] - gd;
-            sd = hit_image[pix] != -1 && gd > 0.f && rd < in.depth_error_max;  // rtg_loss_l1's depth pixels (signed error)
+            sd = frame_depth_pixel(hit_image[pix], gd, rd, in.depth_error_max);  // rtg_loss_l1's depth pixels
         }
         if constexpr (EXPOSURE) {
             // Each term is reduced as soon as it is formed (double warp butterfly, lane 0 stores the warp's sum), the depth

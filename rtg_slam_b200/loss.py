@@ -2,8 +2,9 @@
 
 Drop-in for the colour / depth terms of `Mapping.loss_update` (SLAM/multiprocess/mapper.py:402-431,444-451; `l1_loss` of
 utils/loss_utils.py:27-31). The reference evaluates them with ~25 eager kernels (boolean-mask compactions included) and
-autograd builds the same number again in the backward; here two kernels produce the loss *and* dL/d(colour), dL/d(depth),
-which autograd hands straight to the rasterizer backward."""
+autograd builds the same number again in the backward; here three kernels produce the loss *and* dL/d(colour), dL/d(depth),
+which autograd hands straight to the rasterizer backward. Their sums are added in a fixed order: two calls on the same
+inputs give the same bits."""
 from __future__ import annotations
 
 import ctypes as C
@@ -27,17 +28,11 @@ def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
-def _l1_inputs(render, depth, depth_index, gt_color, gt_depth, render_mask):
-    """The checked, contiguous inputs of both L1 entries: (render, depth, depth_index, gt_color, gt_depth, mask, H, W,
-    channels_last)."""
-    for name, t in (("render", render), ("depth", depth), ("gt_color", gt_color), ("gt_depth", gt_depth)):
-        if not t.is_cuda or t.dtype != torch.float32:
-            raise TypeError(f"{name} must be a CUDA float32 tensor")
-    if depth_index.dtype != torch.int32:
-        raise TypeError("depth_index must be int32 (the rasterizer's depth_index_map)")
-    _, H, W = render.shape
-    render, depth, depth_index = render.contiguous(), depth.contiguous(), depth_index.contiguous()
-    gt_color, gt_depth = gt_color.contiguous(), gt_depth.contiguous()
+def frame_targets(gt_color, gt_depth, render_mask, H, W):
+    """A measured H x W frame as the native losses and pose steps read it: (gt_color, gt_depth, mask, channels_last).
+    gt_color (H,W,3) (channels_last = 1) or (3,H,W) (0) and gt_depth with H*W elements, both CUDA float32, come back
+    detached and contiguous; render_mask (H*W elements, any dtype, nonzero = selected) as contiguous uint8 on their device,
+    or None."""
     if gt_color.shape == (H, W, 3):
         channels_last = 1
     elif gt_color.shape == (3, H, W):
@@ -46,72 +41,66 @@ def _l1_inputs(render, depth, depth_index, gt_color, gt_depth, render_mask):
         raise ValueError("gt_color must be (H,W,3) or (3,H,W)")
     if gt_depth.numel() != H * W:
         raise ValueError("gt_depth must have H*W elements")
+    for name, t in (("gt_color", gt_color), ("gt_depth", gt_depth)):
+        if not t.is_cuda or t.dtype != torch.float32:
+            raise TypeError(f"{name} must be a CUDA float32 tensor")
     mask = None
     if render_mask is not None:
-        mask = render_mask.to(torch.uint8).contiguous() if render_mask.dtype != torch.uint8 else render_mask.contiguous()
-        if mask.numel() != H * W:
+        if render_mask.numel() != H * W:
             raise ValueError("render_mask must have H*W elements")
-    return render, depth, depth_index, gt_color, gt_depth, mask, H, W, channels_last
+        mask = render_mask.detach().to(device=gt_depth.device, dtype=torch.uint8).contiguous()
+    return gt_color.detach().contiguous(), gt_depth.detach().contiguous(), mask, channels_last
 
 
-class _FusedL1(torch.autograd.Function):
+class _FusedLoss(torch.autograd.Function):
+    """The frame loss and its gradients from one native call: rtg_loss_mapping if `mapping` (with the normal term when
+    `normal` is given), else rtg_loss_l1_exposure if `exposure` is given, else rtg_loss_l1. Returns (loss, parts)."""
+
     @staticmethod
-    def forward(ctx, render, depth, depth_index, gt_color, gt_depth, render_mask, color_weight, depth_weight, depth_error_max):
+    def forward(ctx, render, depth, normal, exposure, depth_index, gt_color, gt_depth, gt_normal, render_mask, weights, mapping):
         L = _lib.lib()
         dev = render.device
-        render, depth, depth_index, gt_color, gt_depth, mask, H, W, channels_last = _l1_inputs(render, depth, depth_index, gt_color,
-                                                                                               gt_depth, render_mask)
-        g_color = torch.empty_like(render)
-        g_depth = torch.empty_like(depth)
-        out = torch.empty(4, dtype=torch.float32, device=dev)
-        check(L.rtg_loss_l1(_p(render), _p(depth), _p(depth_index), _p(gt_color), _p(gt_depth), _p(mask), H, W, channels_last,
-                            float(color_weight), float(depth_weight), float(depth_error_max), _p(g_color), _p(g_depth), _p(out),
-                            _p(_ws(dev)), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "rtg_loss_l1")
-        ctx.save_for_backward(g_color, g_depth)
+        for name, t in (("render", render), ("depth", depth)):
+            if not t.is_cuda or t.dtype != torch.float32:
+                raise TypeError(f"{name} must be a CUDA float32 tensor")
+        if depth_index.dtype != torch.int32:
+            raise TypeError("depth_index must be int32 (the rasterizer's depth_index_map)")
+        _, H, W = render.shape
+        render, depth, depth_index = render.contiguous(), depth.contiguous(), depth_index.contiguous()
+        gt_color, gt_depth, mask, channels_last = frame_targets(gt_color, gt_depth, render_mask, H, W)
+        color_weight, depth_weight, normal_weight, depth_error_max = (float(w) for w in weights)
+        g_color, g_depth, g_normal, g_exposure = torch.empty_like(render), torch.empty_like(depth), None, None
+        out = torch.empty(8 if mapping else 4, dtype=torch.float32, device=dev)
+        frame = (_p(depth_index), _p(gt_color), _p(gt_depth))
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        if mapping:
+            if normal is not None:
+                normal, gt_normal = normal.contiguous(), gt_normal.contiguous()
+                if normal.shape != (3, H, W) or gt_normal.shape != (H, W, 3):
+                    raise ValueError("normal must be (3,H,W) and gt_normal (H,W,3)")
+                g_normal = torch.empty_like(render)
+            check(L.rtg_loss_mapping(_p(render), _p(depth), _p(normal), *frame, _p(gt_normal), _p(mask), H, W, channels_last,
+                                     color_weight, depth_weight, normal_weight, depth_error_max, _p(g_color), _p(g_depth),
+                                     _p(g_normal), _p(out), _p(_ws(dev)), stream), "rtg_loss_mapping")
+        elif exposure is None:
+            check(L.rtg_loss_l1(_p(render), _p(depth), *frame, _p(mask), H, W, channels_last, color_weight, depth_weight,
+                                depth_error_max, _p(g_color), _p(g_depth), _p(out), _p(_ws(dev)), stream), "rtg_loss_l1")
+        else:
+            if not exposure.is_cuda or exposure.dtype != torch.float32 or exposure.shape != (2,):
+                raise TypeError("exposure must be a (2,) CUDA float32 tensor")
+            exposure = exposure.contiguous()
+            g_exposure = torch.empty(2, dtype=torch.float32, device=dev)
+            check(L.rtg_loss_l1_exposure(_p(render), _p(depth), *frame, _p(mask), H, W, channels_last, color_weight, depth_weight,
+                                         depth_error_max, _p(exposure), _p(g_color), _p(g_depth), _p(g_exposure), _p(out),
+                                         _p(_ws(dev)), stream), "rtg_loss_l1_exposure")
+        ctx.save_for_backward(g_color, g_depth, g_normal, g_exposure)
         ctx.mark_non_differentiable(out)
         return out[0], out
 
     @staticmethod
     def backward(ctx, grad_loss, _grad_parts):
-        g_color, g_depth = ctx.saved_tensors
-        return g_color * grad_loss, g_depth * grad_loss, None, None, None, None, None, None, None
-
-
-_EXPOSURE_WS = {}
-
-
-class _FusedL1Exposure(torch.autograd.Function):
-    """_FusedL1 of a render seen under the frame exposure (a, b): rtg_loss_l1_exposure, which also returns dL/d(a, b)."""
-
-    @staticmethod
-    def forward(ctx, render, depth, depth_index, gt_color, gt_depth, render_mask, color_weight, depth_weight, depth_error_max,
-                exposure):
-        L = _lib.lib()
-        dev = render.device
-        render, depth, depth_index, gt_color, gt_depth, mask, H, W, channels_last = _l1_inputs(render, depth, depth_index, gt_color,
-                                                                                               gt_depth, render_mask)
-        if not exposure.is_cuda or exposure.dtype != torch.float32 or exposure.shape != (2,):
-            raise TypeError("exposure must be a (2,) CUDA float32 tensor")
-        exposure = exposure.contiguous()
-        idx = dev.index if dev.index is not None else torch.cuda.current_device()
-        if idx not in _EXPOSURE_WS:
-            _EXPOSURE_WS[idx] = torch.zeros(L.rtg_loss_l1_exposure_workspace_bytes(), dtype=torch.uint8, device=torch.device("cuda", idx))
-        g_color = torch.empty_like(render)
-        g_depth = torch.empty_like(depth)
-        g_exposure = torch.empty(2, dtype=torch.float32, device=dev)
-        out = torch.empty(4, dtype=torch.float32, device=dev)
-        check(L.rtg_loss_l1_exposure(_p(render), _p(depth), _p(depth_index), _p(gt_color), _p(gt_depth), _p(mask), H, W, channels_last,
-                                     float(color_weight), float(depth_weight), float(depth_error_max), _p(exposure), _p(g_color),
-                                     _p(g_depth), _p(g_exposure), _p(out), _p(_EXPOSURE_WS[idx]),
-                                     C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "rtg_loss_l1_exposure")
-        ctx.save_for_backward(g_color, g_depth, g_exposure)
-        ctx.mark_non_differentiable(out)
-        return out[0], out
-
-    @staticmethod
-    def backward(ctx, grad_loss, _grad_parts):
-        g_color, g_depth, g_exposure = ctx.saved_tensors
-        return g_color * grad_loss, g_depth * grad_loss, None, None, None, None, None, None, None, g_exposure * grad_loss
+        grads = tuple(None if g is None else g * grad_loss for g in ctx.saved_tensors)  # render, depth, normal, exposure
+        return grads + (None,) * 7
 
 
 def l1_color_depth_loss(render_output, gt_color, gt_depth, render_mask=None, color_weight=0.8, depth_weight=1.0,
@@ -121,62 +110,8 @@ def l1_color_depth_loss(render_output, gt_color, gt_depth, render_mask=None, col
     `exposure`: None, or a (2,) CUDA float32 tensor (a, b): the colour residual becomes e^a render + b - gt_color
     (rtg_loss_l1_exposure) and the loss is differentiable with respect to the render and to `exposure`, so that a keyframe
     can be fitted under its camera's brightness without baking it into the map."""
-    if exposure is not None:
-        return _FusedL1Exposure.apply(render_output["render"], render_output["depth"], render_output["depth_index_map"], gt_color,
-                                      gt_depth, render_mask, color_weight, depth_weight, depth_error_max, exposure)
-    return _FusedL1.apply(render_output["render"], render_output["depth"], render_output["depth_index_map"], gt_color, gt_depth,
-                          render_mask, color_weight, depth_weight, depth_error_max)
-
-
-# ----------------------------------------------------------------------------- full mapping loss (SURVEY 8(f) #1)
-class _FusedMapping(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, render, depth, normal, depth_index, gt_color, gt_depth, gt_normal, render_mask, color_weight, depth_weight,
-                normal_weight, depth_error_max):
-        L = _lib.lib()
-        dev = render.device
-        _, H, W = render.shape
-        render, depth, depth_index = render.contiguous(), depth.contiguous(), depth_index.contiguous()
-        gt_color, gt_depth = gt_color.contiguous(), gt_depth.contiguous()
-        if gt_color.shape == (H, W, 3):
-            channels_last = 1
-        elif gt_color.shape == (3, H, W):
-            channels_last = 0
-        else:
-            raise ValueError("gt_color must be (H,W,3) or (3,H,W)")
-        for name, t in (("render", render), ("depth", depth), ("gt_color", gt_color), ("gt_depth", gt_depth)):
-            if not t.is_cuda or t.dtype != torch.float32:
-                raise TypeError(f"{name} must be a CUDA float32 tensor")
-        if depth_index.dtype != torch.int32:
-            raise TypeError("depth_index must be int32 (the rasterizer's depth_index_map)")
-        use_normal = normal_weight > 0 and normal is not None and gt_normal is not None
-        if use_normal:
-            normal, gt_normal = normal.contiguous(), gt_normal.contiguous()
-            if normal.shape != (3, H, W) or gt_normal.shape != (H, W, 3):
-                raise ValueError("normal must be (3,H,W) and gt_normal (H,W,3)")
-        mask = None
-        if render_mask is not None:
-            mask = render_mask.to(torch.uint8).contiguous() if render_mask.dtype != torch.uint8 else render_mask.contiguous()
-            if mask.numel() != H * W:
-                raise ValueError("render_mask must have H*W elements")
-        g_color, g_depth = torch.empty_like(render), torch.empty_like(depth)
-        g_normal = torch.empty_like(render) if use_normal else None
-        out = torch.empty(8, dtype=torch.float32, device=dev)
-        check(L.rtg_loss_mapping(_p(render), _p(depth), _p(normal if use_normal else None), _p(depth_index), _p(gt_color), _p(gt_depth),
-                                 _p(gt_normal if use_normal else None), _p(mask), H, W, channels_last, float(color_weight),
-                                 float(depth_weight), float(normal_weight) if use_normal else 0.0, float(depth_error_max), _p(g_color),
-                                 _p(g_depth), _p(g_normal), _p(out), _p(_ws(dev)), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-              "rtg_loss_mapping")
-        ctx.use_normal = use_normal
-        ctx.save_for_backward(g_color, g_depth, *([g_normal] if use_normal else []))
-        ctx.mark_non_differentiable(out)
-        return out[0], out
-
-    @staticmethod
-    def backward(ctx, grad_loss, _grad_parts):
-        saved = ctx.saved_tensors
-        gn = saved[2] * grad_loss if ctx.use_normal else None
-        return (saved[0] * grad_loss, saved[1] * grad_loss, gn) + (None,) * 9
+    return _FusedLoss.apply(render_output["render"], render_output["depth"], None, exposure, render_output["depth_index_map"],
+                            gt_color, gt_depth, None, render_mask, (color_weight, depth_weight, 0.0, depth_error_max), False)
 
 
 _SSIM_WS = {}
@@ -252,15 +187,16 @@ def mapping_loss(render_output, image_input, render_mask=None, color_weight=0.8,
     """The image-space part of `Mapping.loss_update` (SLAM/multiprocess/mapper.py:402-451): colour L1 on the render mask,
     depth L1 on the valid mask, cosine normal loss, and -- only without a render mask, as in the reference -- the SSIM
     term. `render_output`: dict of Renderer.render; `image_input`: dict with "color_map" (H,W,3), "depth_map" (H,W[,1]),
-    "normal_map" (H,W,3). Colour, depth and normal terms and their gradients come from two fused kernels, the SSIM term
+    "normal_map" (H,W,3). Colour, depth and normal terms and their gradients come from three fused kernels, the SSIM term
     (which the shipped flows never reach: both call sites pass a render mask) from three more (`ssim_loss`).
     Returns (total_loss, parts): parts is a device tensor {total, colour, depth, n_depth, normal, n_normal, ssim, 0} --
     read it back once with `report_losses` instead of six `.item()` calls (mapper.py:459-466)."""
-    nrm = render_output.get("normal") if normal_weight > 0 else None
-    gtn = image_input.get("normal_map") if normal_weight > 0 else None
-    loss, parts = _FusedMapping.apply(render_output["render"], render_output["depth"], nrm, render_output["depth_index_map"],
-                                      image_input["color_map"], image_input["depth_map"], gtn, render_mask, color_weight, depth_weight,
-                                      normal_weight, depth_error_max)
+    nrm, gtn = render_output.get("normal"), image_input.get("normal_map")
+    if not (normal_weight > 0 and nrm is not None and gtn is not None):
+        nrm, gtn, normal_weight = None, None, 0.0
+    loss, parts = _FusedLoss.apply(render_output["render"], render_output["depth"], nrm, None, render_output["depth_index_map"],
+                                   image_input["color_map"], image_input["depth_map"], gtn, render_mask,
+                                   (color_weight, depth_weight, normal_weight, depth_error_max), True)
     if render_mask is None and ssim_weight > 0:
         gt = image_input["color_map"]
         gt = gt.permute(2, 0, 1) if gt.shape[-1] == 3 and gt.dim() == 3 and gt.shape[0] != 3 else gt

@@ -40,7 +40,7 @@ import torch
 
 from . import _lib, rasterizer
 from ._lib import RtgPoseAdam, RtgPoseGN, check
-from .loss import l1_color_depth_loss
+from .loss import frame_targets, l1_color_depth_loss
 from .optim import FusedAdam
 from .rasterizer import CapacityOverflow, GaussianRasterizationSettings, _forward_native, _make_view, rasterize_gaussians
 from .render import Renderer
@@ -135,28 +135,13 @@ def downsample_frame(gt_color, gt_depth, s, render_mask=None, tile_mask=None):
     if s < 2:
         raise ValueError("s must be >= 2")
     H, W = int(gt_depth.shape[-2]), int(gt_depth.shape[-1])
-    if gt_depth.numel() != H * W:
-        raise ValueError("gt_depth must be (H,W) or (1,H,W)")
-    if gt_color.shape == (H, W, 3):
-        channels_last = 1
-    elif gt_color.shape == (3, H, W):
-        channels_last = 0
-    else:
-        raise ValueError("gt_color must be (H,W,3) or (3,H,W)")
-    for name, t in (("gt_color", gt_color), ("gt_depth", gt_depth)):
-        if not t.is_cuda or t.dtype != torch.float32:
-            raise TypeError(f"{name} must be a CUDA float32 tensor")
+    gt_color, gt_depth, mask, channels_last = frame_targets(gt_color, gt_depth, render_mask, H, W)
     dev = gt_depth.device
     Hs, Ws = H // s, W // s
-    gt_color, gt_depth = gt_color.detach().contiguous(), gt_depth.detach().contiguous()
     color = torch.empty((3, Hs, Ws), dtype=torch.float32, device=dev)
     depth = torch.empty((Hs, Ws), dtype=torch.float32, device=dev)
-    mask = mask_out = tmask = tmask_out = None
-    if render_mask is not None:
-        if render_mask.numel() != H * W:
-            raise ValueError("render_mask must have H*W elements")
-        mask = render_mask.detach().to(device=dev, dtype=torch.uint8).contiguous()
-        mask_out = torch.empty_like(depth, dtype=torch.uint8)
+    mask_out = None if mask is None else torch.empty_like(depth, dtype=torch.uint8)
+    tmask = tmask_out = None
     if tile_mask is not None:
         if not tile_mask.is_cuda or tile_mask.dtype != torch.int32:
             raise TypeError("tile_mask must be a CUDA int32 tensor")
@@ -242,23 +227,7 @@ class PoseRefiner:
             raise ValueError('robust must be None or "huber"')
         dev, pose, projection, view, proj, campos, rs, g = self._setup(camera, gaussian_data, requires_grad=False)
         H, W = int(rs.image_height), int(rs.image_width)
-        gt_color, gt_depth = gt_color.detach().contiguous(), gt_depth.detach().contiguous()
-        if gt_color.shape == (H, W, 3):
-            channels_last = 1
-        elif gt_color.shape == (3, H, W):
-            channels_last = 0
-        else:
-            raise ValueError("gt_color must be (H,W,3) or (3,H,W)")
-        if gt_depth.numel() != H * W:
-            raise ValueError("gt_depth must have H*W elements")
-        for name, t in (("gt_color", gt_color), ("gt_depth", gt_depth)):
-            if not t.is_cuda or t.dtype != torch.float32:
-                raise TypeError(f"{name} must be a CUDA float32 tensor")
-        mask = None
-        if render_mask is not None:
-            mask = render_mask.detach().to(torch.uint8).contiguous()
-            if mask.numel() != H * W:
-                raise ValueError("render_mask must have H*W elements")
+        gt_color, gt_depth, mask, channels_last = frame_targets(gt_color, gt_depth, render_mask, H, W)
         P = int(g["xyz"].shape[0])
         L = _lib.lib()
         scratch_bytes = L.rtg_splat_pose_gn_scratch_bytes if exposure is None else L.rtg_splat_pose_gn_exposure_scratch_bytes

@@ -275,6 +275,10 @@ def test_mapping_loss_with_normal_and_ssim_terms(cuda_device, use_mask):
     got = [t.grad.clone() for t in (render, depth, normal)]
     for t in (render, depth, normal):
         t.grad = None
+    _, parts2 = mapping_loss({"render": render, "depth": depth, "normal": normal, "depth_index_map": depth_index},
+                             {"color_map": gt_color, "depth_map": gt_depth, "normal_map": gt_normal}, render_mask=mask,
+                             depth_error_max=0.1, **w)
+    assert torch.equal(parts, parts2)  # fixed-order sums: the same bits from call to call
     # the reference's expressions
     image, d, n, di = render.permute(1, 2, 0), depth.permute(1, 2, 0), normal.permute(1, 2, 0), depth_index.permute(1, 2, 0)
     ssim_loss = torch.zeros((), device=dev)

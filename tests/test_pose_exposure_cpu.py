@@ -283,26 +283,46 @@ def test_pose_gn_step_exposure_validates_before_touching_cuda():
 
 
 def test_loss_l1_exposure_validates_before_touching_cuda():
+    """rtg_loss_l1_exposure, rtg_loss_l1 and rtg_loss_mapping share one host validation, each with its own extra rule."""
     from rtg_slam_b200 import _lib
     L = _lib.lib()
     ok = C.c_void_p(256)
-    names = ("render", "depth", "depth_index", "gt_color", "gt_depth", "mask", "exposure", "dL_dcolor", "dL_ddepth", "dL_dexposure",
-             "loss_out", "ws")
+    names = ("render", "depth", "normal", "depth_index", "gt_color", "gt_depth", "gt_normal", "mask", "exposure", "dL_dcolor",
+             "dL_ddepth", "dL_dnormal", "dL_dexposure", "loss_out", "ws")
 
-    def call(H=16, W=16, **over):
+    def args(H, W, over):
         p = {k: ok for k in names}
         p.update(over)
+        return p, H, W
+
+    def exposure(H=16, W=16, **over):
+        p, H, W = args(H, W, over)
         return L.rtg_loss_l1_exposure(p["render"], p["depth"], p["depth_index"], p["gt_color"], p["gt_depth"], p["mask"], H, W, 0,
                                       0.8, 1.0, 0.1, p["exposure"], p["dL_dcolor"], p["dL_ddepth"], p["dL_dexposure"], p["loss_out"],
                                       p["ws"], None)
-    for kw in (dict(H=0), dict(W=-1)):
-        assert call(**kw) == -1 and b"H and W must be >= 1" in L.rtg_last_error(), kw
-    for k in ("render", "depth", "depth_index", "gt_color", "gt_depth", "dL_dcolor", "dL_ddepth", "loss_out", "ws"):
-        assert call(**{k: None}) == -1 and b"NULL pointer" in L.rtg_last_error(), k
+
+    def l1(H=16, W=16, **over):
+        p, H, W = args(H, W, over)
+        return L.rtg_loss_l1(p["render"], p["depth"], p["depth_index"], p["gt_color"], p["gt_depth"], p["mask"], H, W, 0, 0.8, 1.0,
+                             0.1, p["dL_dcolor"], p["dL_ddepth"], p["loss_out"], p["ws"], None)
+
+    def mapping(H=16, W=16, normal_weight=0.1, **over):
+        p, H, W = args(H, W, over)
+        return L.rtg_loss_mapping(p["render"], p["depth"], p["normal"], p["depth_index"], p["gt_color"], p["gt_depth"], p["gt_normal"],
+                                  p["mask"], H, W, 0, 0.8, 1.0, normal_weight, 0.1, p["dL_dcolor"], p["dL_ddepth"], p["dL_dnormal"],
+                                  p["loss_out"], p["ws"], None)
+
+    for call, who in ((exposure, b"rtg_loss_l1_exposure"), (l1, b"rtg_loss_l1:"), (mapping, b"rtg_loss_mapping")):
+        for kw in (dict(H=0), dict(W=-1)):
+            assert call(**kw) == -1 and b"H and W must be >= 1" in L.rtg_last_error(), (who, kw)
+        for k in ("render", "depth", "depth_index", "gt_color", "gt_depth", "dL_dcolor", "dL_ddepth", "loss_out", "ws"):
+            assert call(**{k: None}) == -1 and b"NULL pointer" in L.rtg_last_error(), (who, k)
+        assert call(mask=None, ws=C.c_void_p(260)) == -1 and b"8-byte aligned" in L.rtg_last_error(), who
+        assert who in L.rtg_last_error()
     for k in ("exposure", "dL_dexposure"):
-        assert call(**{k: None}) == -1 and b"NULL exposure" in L.rtg_last_error(), k
-    assert call(ws=C.c_void_p(260)) == -1 and b"8-byte aligned" in L.rtg_last_error()
-    assert b"rtg_loss_l1_exposure" in L.rtg_last_error()
+        assert exposure(**{k: None}) == -1 and b"NULL exposure" in L.rtg_last_error(), k
+    for k in ("normal", "gt_normal", "dL_dnormal"):
+        assert mapping(**{k: None}) == -1 and b"normal_weight > 0 needs" in L.rtg_last_error(), k
 
 
 def test_refiners_reject_a_malformed_exposure():

@@ -122,6 +122,46 @@ def test_fused_adam_matches_torch(cuda_device):
     assert torch.equal(before, pa[0])
 
 
+def test_fused_adam_at_map_size_matches_float64_torch(cuda_device):
+    """The six groups at P = 1,000,003 plus a parameter at a storage offset of one float, against torch.optim.Adam in
+    float64 from the same float32 start. adam_kernel caps its grid at 2112 x 256 threads of four floats: features_rest
+    (45 M elements) takes 21 grid-stride passes; the (P,1), (P,3) and (P,15,3) groups have numel % 4 != 0, so their
+    scalar tail runs after the float4 body; the offset view is not 16-byte aligned and takes the scalar path throughout."""
+    from rtg_slam_b200.optim import FusedAdam
+    dev = cuda_device
+    P = 1_000_003
+    gen = torch.Generator(device=dev).manual_seed(11)
+    shapes = [(P, 3), (P, 1, 3), (P, 15, 3), (P, 1), (P, 3), (P, 4)]
+    lrs = [1e-3, 5e-4, 5e-4 / 20.0, 0.0, 4e-3, 1e-3]
+    pa = [torch.randn(s, device=dev, generator=gen).requires_grad_(True) for s in shapes]
+    base = torch.randn(P * 3 + 1, device=dev, generator=gen)
+    before = base[:1].clone()
+    pa.append(base[1:].view(P, 3).requires_grad_(True))              # a contiguous view one float into its storage
+    lrs.append(2e-3)
+    assert pa[-1].is_contiguous() and pa[-1].data_ptr() % 16 == 4
+    assert [p.numel() % 4 for p in pa[:6]] == [1, 1, 3, 3, 1, 0]
+    pb = [p.detach().double().requires_grad_(True) for p in pa]
+    oa = FusedAdam([{"params": [p], "lr": lr} for p, lr in zip(pa, lrs)], lr=0.0, eps=1e-15)
+    ob = torch.optim.Adam([{"params": [p], "lr": lr} for p, lr in zip(pb, lrs)], lr=0.0, eps=1e-15)
+    start = [p.detach().clone() for p in pa]
+    rng = np.random.default_rng(2)
+    for it in range(3):
+        for p, q in zip(pa, pb):
+            gr = torch.randn(p.shape, device=dev, generator=gen) * float(10 ** rng.uniform(-5, 0))
+            gr.view(-1)[::7] = 0                                         # exact zeros stay harmless with eps = 1e-15
+            p.grad, q.grad = gr, gr.double()
+        oa.step(); ob.step()
+        oa.zero_grad(set_to_none=True); ob.zero_grad(set_to_none=True)
+    for k, (p, q, lr, p0) in enumerate(zip(pa, pb, lrs, start)):
+        e = float((p.detach().double() - q.detach()).abs().max() / q.detach().abs().max())
+        assert e < 1e-5, (k, e)
+        if lr == 0.0:
+            assert torch.equal(p.detach(), p0)                          # the lr = 0 group does not move, bit for bit
+        else:
+            assert not torch.equal(p.detach(), p0), k
+    assert torch.equal(base[:1], before)                                 # the float in front of the view is not written
+
+
 def test_renderer_api(cuda_device):
     """Renderer.render returns the reference's dictionary; the normal map equals normal[depth_index_map]."""
     from rtg_slam_b200.render import Renderer

@@ -34,7 +34,10 @@ def _get_normal(scaling_raw, rotation_raw):
     return n / (torch.norm(n, dim=-1, keepdim=True) + 1e-8)
 
 
-@pytest.mark.parametrize("P,with_attach,use_radii", [(5003, True, True), (4096, False, False), (37, True, False)])
+# 300,007 and 1,000,003 rows: map_adam_kernel launches one wave of resident CTAs (at most 1056 x 8 warps on 132 SMs), so
+# its grid-stride loop makes a second and later pass over the 32-row blocks, and the last block is partial
+@pytest.mark.parametrize("P,with_attach,use_radii", [(5003, True, True), (4096, False, False), (37, True, False), (300_007, False, False),
+                                                     (1_000_003, True, True)])
 def test_map_step_matches_torch_activations_and_adam(cuda_device, P, with_attach, use_radii):
     from rtg_slam_b200.mapoptim import MapOptimizer
     dev = cuda_device
@@ -51,30 +54,45 @@ def test_map_step_matches_torch_activations_and_adam(cuda_device, P, with_attach
                  "xyz": raw["xyz"] + 0.01 * torch.randn_like(raw["xyz"]), "rotation_raw": raw["rotation"] + 0.02 * torch.randn_like(raw["rotation"])}
     iters = 10
 
-    def image_loss(d):  # any smooth function of the activated tensors stands in for render + loss
+    def image_loss(d):  # any smooth function of the activated tensors stands in for render + loss (reference_flow repeats it)
         return sum((W[k] * (d[k] ** 2 + d[k])).sum() for k in W)
 
-    # ---- reference flow
-    p = {k: torch.nn.Parameter(v.clone()) for k, v in raw.items()}
-    groups = [{"params": [p["xyz"]], "lr": LRS["xyz"]}, {"params": [p["features_dc"]], "lr": LRS["f_dc"]},
-              {"params": [p["features_rest"]], "lr": LRS["f_rest"]}, {"params": [p["opacity"]], "lr": LRS["opacity"]},
-              {"params": [p["scaling"]], "lr": LRS["scaling"]}, {"params": [p["rotation"]], "lr": LRS["rotation"]}]
-    ref_opt = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
-    conf_ref = torch.zeros(P, device=dev)
-    for _ in range(iters):
-        d = dict(xyz=p["xyz"], shs=torch.cat((p["features_dc"], p["features_rest"]), dim=1), opacity=torch.sigmoid(p["opacity"]),
-                 scales=torch.exp(p["scaling"]), rotations=F.normalize(p["rotation"]))
-        loss = image_loss(d)
-        if with_attach:
-            m = (torch.sigmoid(init_stat["opacity"]) < 0.9).squeeze()
-            l2 = lambda a, b: ((a - b) ** 2).mean()
-            if m.sum() > 0:
-                loss = loss + 1000 * (l2(p["scaling"][m], init_stat["scaling"][m]) + l2(p["xyz"][m], init_stat["xyz"][m])
-                                      + l2(p["rotation"][m], init_stat["rotation_raw"][m]))
-        loss.backward()
-        ref_opt.step()
-        conf_ref[(p["features_dc"].grad.abs() != 0).any(dim=-1).squeeze(-1)] += 1
-        ref_opt.zero_grad(set_to_none=True)
+    # ---- reference flow, in float32 (the reference's own precision) and in float64
+    def reference_flow(dtype):
+        p = {k: torch.nn.Parameter(v.to(dtype, copy=True)) for k, v in raw.items()}
+        Wd, ist = {k: v.to(dtype) for k, v in W.items()}, {k: v.to(dtype) for k, v in init_stat.items()}
+        groups = [{"params": [p["xyz"]], "lr": LRS["xyz"]}, {"params": [p["features_dc"]], "lr": LRS["f_dc"]},
+                  {"params": [p["features_rest"]], "lr": LRS["f_rest"]}, {"params": [p["opacity"]], "lr": LRS["opacity"]},
+                  {"params": [p["scaling"]], "lr": LRS["scaling"]}, {"params": [p["rotation"]], "lr": LRS["rotation"]}]
+        ref_opt = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
+        conf_ref = torch.zeros(P, device=dev)
+        for _ in range(iters):
+            d = dict(xyz=p["xyz"], shs=torch.cat((p["features_dc"], p["features_rest"]), dim=1), opacity=torch.sigmoid(p["opacity"]),
+                     scales=torch.exp(p["scaling"]), rotations=F.normalize(p["rotation"]))
+            loss = sum((Wd[k] * (d[k] ** 2 + d[k])).sum() for k in Wd)
+            if with_attach:
+                m = (torch.sigmoid(ist["opacity"]) < 0.9).squeeze()
+                l2 = lambda a, b: ((a - b) ** 2).mean()
+                if m.sum() > 0:
+                    loss = loss + 1000 * (l2(p["scaling"][m], ist["scaling"][m]) + l2(p["xyz"][m], ist["xyz"][m])
+                                          + l2(p["rotation"][m], ist["rotation_raw"][m]))
+            loss.backward()
+            ref_opt.step()
+            conf_ref[(p["features_dc"].grad.abs() != 0).any(dim=-1).squeeze(-1)] += 1
+            ref_opt.zero_grad(set_to_none=True)
+        return p, conf_ref
+    p, conf_ref = reference_flow(torch.float32)
+    p64, _ = reference_flow(torch.float64)
+    # Rows on which float32 rounding alone moves the reference by more than a tenth of the bound: Adam with eps = 1e-15
+    # turns a gradient component that cancels to rounding level into a full step of either sign. At a million rows a
+    # rotation row or so does that (float32 torch 1e-3 from float64 there); the kernel is held to float64 on them instead.
+    ill = torch.zeros(P, dtype=torch.bool, device=dev)
+    for k in p:
+        top = float(p64[k].detach().abs().max())
+        ill |= (p[k].detach().double() - p64[k].detach()).abs().reshape(P, -1).amax(1) > 1e-6 * top
+    print(f"P={P}: {int(ill.sum())} rows where float32 torch is more than 1e-6 from float64")
+    assert int(ill.sum()) <= P // 100_000
+    ok = ~ill
 
     # ---- fused flow
     conf = torch.zeros(P, device=dev)
@@ -93,7 +111,7 @@ def test_map_step_matches_torch_activations_and_adam(cuda_device, P, with_attach
         assert opt.xyz.grad is None
 
     def rel(a, b):
-        return float((a - b).abs().max()) / (float(b.abs().max()) + 1e-12)
+        return float((a[ok] - b[ok]).abs().max()) / (float(b.abs().max()) + 1e-12)
     got = dict(xyz=opt.xyz.detach(), features_dc=opt.features_dc, features_rest=opt.features_rest, opacity=opt.opacity_raw,
                scaling=opt.scaling_raw, rotation=opt.rotation_raw)
     for k in got:
@@ -101,6 +119,10 @@ def test_map_step_matches_torch_activations_and_adam(cuda_device, P, with_attach
         assert moved > 0, k
         e = rel(got[k], p[k].detach())
         assert e < 1e-5, (k, e, moved)
+        # the ill-conditioned rows: no further from float64 than a few times float32 torch is
+        want, ref = p64[k].detach()[ill], p[k].detach()[ill].double()
+        top = float(p64[k].detach().abs().max())
+        assert bool(((got[k][ill].double() - want).abs() <= 4 * (ref - want).abs() + 1e-5 * top).all()), k
     # activated tensors for the next render, and the normal
     assert rel(opt.scales.detach(), torch.exp(p["scaling"].detach())) < 1e-5
     assert rel(opt.rotations.detach(), F.normalize(p["rotation"].detach())) < 1e-5
@@ -108,7 +130,7 @@ def test_map_step_matches_torch_activations_and_adam(cuda_device, P, with_attach
     n_ref = _get_normal(p["scaling"].detach(), p["rotation"].detach())
     same_axis = torch.argmin(opt.scales.detach(), 1) == torch.argmin(torch.exp(p["scaling"].detach()), 1)
     assert float(same_axis.float().mean()) > 0.999
-    assert float((opt.normal - n_ref)[same_axis].abs().max()) < 1e-4
+    assert float((opt.normal - n_ref)[same_axis & ok].abs().max()) < 1e-4
     assert torch.equal(conf, conf_ref) and float(conf.max()) == iters
     if with_attach:
         m = (torch.sigmoid(init_stat["opacity"]) < 0.9).squeeze()

@@ -37,7 +37,8 @@ def _check_knn(d2, idx, want_d2, query, ref, K):
     assert np.all(idx[~fin] == 2**31 - 1)
 
 
-@pytest.mark.parametrize("n,K", [(1, 3), (2, 3), (5, 3), (3000, 3), (20_000, 6), (20_000, 8)])
+@pytest.mark.parametrize("n,K", [(1, 3), (2, 3), (5, 3), (3000, 3), (20_000, 6), (20_000, 8), (5000, 1), (5000, 2), (5000, 4),
+                                 (5000, 5), (5000, 7)])
 def test_knn_self_matches_brute_force(cuda_device, n, K):
     pts = _surface_points(max(n, 100), seed=3)[:n]
     t = torch.from_numpy(pts).to(cuda_device)
@@ -83,6 +84,68 @@ def test_dist_cuda2_large_against_kdtree_and_reference(cuda_device):
     assert (a != b).any(1).mean() < 0.05  # indices differ only among equidistant neighbours (the planted duplicates)
 
 
+@pytest.mark.parametrize("n", [2_200_000, 4_500_000])
+def test_dist_cuda2_at_map_scale_against_kdtree(cuda_device, n):
+    """distCUDA2 on surfel-room centres at map scale. The k-NN grid has min(n / 2, 2^21) cells and the scan of their
+    counts sums 1024 block sums per pass: 2,200,000 points take two passes, 4,500,000 points reach the cap of 2^21 cells
+    and take three. Held to scipy's k-d tree in float64 on a fixed random sample of 20,000 rows plus the first and last
+    1,000 rows."""
+    from scipy.spatial import cKDTree
+    pts = scene.surfel_room(n, seed=5)["xyz"].astype(np.float32)
+    mean, idx = mapsurgery.distCUDA2(torch.from_numpy(pts).to(cuda_device))
+    assert mean.shape == (n,) and idx.shape == (n, 3)
+    rows = np.concatenate([np.arange(1000), np.random.default_rng(n).choice(n, 20_000, replace=False), np.arange(n - 1000, n)])
+    p64 = pts.astype(np.float64)
+    dd, _ = cKDTree(p64).query(p64[rows], k=4)
+    want = (dd[:, 1:] ** 2).mean(1)
+    got = mean.cpu().numpy()[rows]
+    assert np.allclose(got, want, rtol=1e-4, atol=1e-10), float(np.abs(got - want).max())
+    # the indices name three other points at the reported distances
+    ix = idx.cpu().numpy()[rows].astype(np.int64)
+    assert not np.any(ix == rows[:, None])
+    d_ix = ((p64[ix] - p64[rows][:, None, :]) ** 2).sum(-1).mean(1)
+    assert np.allclose(d_ix, want, rtol=1e-4, atol=1e-10)
+
+
+def _degenerate_points(kind, n, rng):
+    """Reference sets on which the k-NN grid takes its special cell-size rules, and the queries asked of them (None: the
+    set itself)."""
+    if kind == "plane":                     # z constant: two extents
+        p = np.concatenate([rng.uniform(-3, 3, (n, 2)), np.full((n, 1), 1.25)], 1)
+    elif kind == "line":                    # y and z constant: one extent
+        p = np.concatenate([rng.uniform(-4, 4, (n, 1)), np.full((n, 1), -0.5), np.full((n, 1), 2.0)], 1)
+    elif kind == "one_point":               # no extent
+        p = np.tile([[0.3, -1.2, 2.0]], (n, 1))
+    elif kind == "two_clusters":            # 100 m apart: a bounding box that is almost all empty
+        p = np.concatenate([rng.normal(0, 0.05, (n // 2, 3)), rng.normal(0, 0.05, (n - n // 2, 3)) + [100.0, 3.0, -2.0]])
+    elif kind == "far_room":                # the surfel room 1000 m from the origin on every axis
+        p = _surface_points(n, seed=21) + 1000.0
+    elif kind == "queries_outside":
+        ref = _surface_points(n, seed=23)
+        q = np.concatenate([ref[:500] + rng.normal(0, 0.01, (500, 3)), rng.uniform(-20, 20, (300, 3)), rng.uniform(-1000, 1000, (200, 3))])
+        return ref, q.astype(np.float32)
+    return p.astype(np.float32), None
+
+
+@pytest.mark.parametrize("kind", ["plane", "line", "one_point", "two_clusters", "far_room", "queries_outside"])
+def test_knn_on_degenerate_geometry_matches_brute_force(cuda_device, kind):
+    """k-NN against the brute-force oracle where the grid's cell size is not the plain cube-root rule: points on a plane,
+    on a line, all identical; two small clusters far apart; a room far from the origin; queries far outside the
+    reference points' box. 10,000 reference points each (the oracle is quadratic); a set queried against itself with and
+    without skip_self (rtg_knn takes skip_self only there)."""
+    rng = np.random.default_rng(["plane", "line", "one_point", "two_clusters", "far_room", "queries_outside"].index(kind))
+    ref, q = _degenerate_points(kind, 10_000, rng)
+    tr = torch.from_numpy(ref).to(cuda_device)
+    tq = tr if q is None else torch.from_numpy(q).to(cuda_device)
+    q = ref if q is None else q
+    for skip in ((False, True) if tq is tr else (False,)):
+        d2, idx = mapsurgery.knn(tq, tr, 4, skip_self=skip)
+        want, _ = ko.knn(q, ref, 4, skip_self=skip)
+        _check_knn(d2, idx, want, q, ref, 4)
+        if skip:
+            assert not np.any(idx.cpu().numpy() == np.arange(len(ref))[:, None])
+
+
 def test_update_geometry_expression_on_our_knn(cuda_device):
     """GaussianPointCloud.update_geometry (gaussian_pointcloud.py:365-405) evaluated with distCUDA2 from this library and
     from the brute-force oracle: same scales / invalid mask."""
@@ -103,7 +166,8 @@ def test_update_geometry_expression_on_our_knn(cuda_device):
     assert np.array_equal(inv_a, inv_b) and np.allclose(s_a, s_b, rtol=1e-5, atol=1e-9)
 
 
-@pytest.mark.parametrize("P", [0, 1, 777, 200_000])
+# 1,048,576 rows fill the 1024 block sums of one pass of the scan over the block sums; 1,048,577 need one more
+@pytest.mark.parametrize("P", [0, 1, 777, 200_000, 1_048_576, 1_048_577])
 def test_soa_delete_remove_cat(cuda_device, P):
     """GaussianPointCloud.delete / remove / cat on the eleven attribute tensors against torch's own boolean indexing."""
     g = torch.Generator(device="cpu").manual_seed(P)
@@ -128,6 +192,25 @@ def test_soa_delete_remove_cat(cuda_device, P):
     for m in (torch.zeros(P, dtype=torch.bool, device=cuda_device), torch.ones(P, dtype=torch.bool, device=cuda_device)):
         d = mapsurgery.delete(params, m)
         assert all(torch.equal(d[k], params[k][~m]) for k in params)
+
+
+def test_compact_past_two_scan_passes(cuda_device):
+    """mapsurgery.compact at 2,500,001 rows (2442 block sums: the scan over them takes three passes of 1024) on rows of
+    1, 3 and 45 words, against torch boolean indexing, bit for bit, with the returned count: a random mask, all kept, none
+    kept, only the last row kept, only the first row kept."""
+    dev = cuda_device
+    P = 2_500_001
+    g = torch.Generator(device=dev).manual_seed(4)
+    ts = [torch.randn(P, generator=g, device=dev), torch.randint(-2**31, 2**31 - 1, (P, 3), generator=g, device=dev, dtype=torch.int32),
+          torch.randn(P, 15, 3, generator=g, device=dev)]
+    one = lambda i: torch.zeros(P, dtype=torch.bool, device=dev).index_fill_(0, torch.tensor([i], device=dev), True)
+    masks = dict(random=torch.rand(P, generator=g, device=dev) < 0.4, all=torch.ones(P, dtype=torch.bool, device=dev),
+                 none=torch.zeros(P, dtype=torch.bool, device=dev), last=one(P - 1), first=one(0))
+    for name, m in masks.items():
+        out, kept = mapsurgery.compact(m, ts)
+        assert kept == int(m.sum()), name
+        for t, o in zip(ts, out):
+            assert o.dtype == t.dtype and torch.equal(o, t[m]), name
 
 
 def test_api_errors(cuda_device):

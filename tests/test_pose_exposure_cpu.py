@@ -1,8 +1,9 @@
 """CPU tests of exposure estimation in the pose refiners: a float64 statement of the eight-unknown Gauss-Newton step
 (pose twist and the frame's exposure (a, b), C^ ~ e^a C + b; reused by the GPU tests), pinned against autograd and, without
-the exposure columns, against the six-unknown statement; a float64 statement of the L1 loss under an exposure against
-autograd; the invariance of (a, b) under the pyramid's block mean; host validation of rtg_splat_pose_gn_step_exposure and
-rtg_loss_l1_exposure and the RtgPoseExposure layout."""
+the exposure columns, against the six-unknown statement; a float64 statement of the three frame losses (L1, L1 under an
+exposure, mapping with the cosine normal term; reused by the GPU tests) against autograd and the eager expressions of the
+mapping loss; the invariance of (a, b) under the pyramid's block mean; host validation of rtg_splat_pose_gn_step_exposure
+and rtg_loss_l1_exposure and the RtgPoseExposure layout."""
 import ctypes as C
 
 import numpy as np
@@ -151,25 +152,46 @@ def test_no_colour_term_leaves_the_exposure():
         assert float((new - want).abs().max()) <= 1e-12
 
 
-# ------------------------------------------------------------------------------------------------ the L1 loss statement
-def l1_exposure_statement(render, depth, hit, gt_color, gt_depth, mask, color_weight, depth_weight, depth_error_max, ab):
-    """rtg_loss_l1_exposure in float64: (loss, colour, depth, n_depth), dL/dC (3, n), dL/ddepth (n), dL/d(a, b).
-    render, gt_color (3, n); depth, gt_depth (n); hit (n) int; mask (n) bool. The depth selection compares in the dtype
-    given (the GPU test passes the float32 error)."""
+# -------------------------------------------------------------------------------------------- the frame loss statement
+def loss_statement(render, depth, hit, gt_color, gt_depth, mask, color_weight, depth_weight, depth_error_max, ab=(0.0, 0.0),
+                   normal=None, gt_normal=None, normal_weight=0.0, depth_near=None):
+    """The three frame losses in float64: rtg_loss_l1 (ab = (0, 0), no normal), rtg_loss_l1_exposure (ab) and
+    rtg_loss_mapping (normal, gt_normal and normal_weight > 0: the cosine normal term). Returns parts [total, colour,
+    depth, n_depth, normal, n_normal, 0, 0] (a list of floats), dL/dC (3, n), dL/ddepth (n), dL/dnormal (3, n) or None,
+    dL/d(a, b) (2).
+    render, gt_color, normal, gt_normal (3, n); depth, gt_depth (n); hit (n) int; mask (n) bool. Colour: mean |e^a C + b -
+    C^| over 3 x the masked pixels. Depth: mean |D - D^| over mask & hit != -1 & D^ > 0 & D - D^ < depth_error_max; the
+    error test is `depth_near` (n) bool if given (the GPU tests pass the float32 comparison the kernel makes). Normal:
+    mean (1 - cos) over mask & hit != -1 & gt_normal != (0, 0, 0), cos = x.y / (max(|x|, 1e-8) max(|y|, 1e-8))
+    (F.cosine_similarity). Every mean over an empty set, and its gradient, is 0. The tensors may live on any device."""
     a, b = float(ab[0]), float(ab[1])
     ea = float(np.exp(a))
+    f64 = dict(dtype=torch.float64, device=render.device)
     r = torch.where(mask[None], ea * render + b - gt_color, torch.zeros_like(render))
     n = float(mask.sum())
     e = depth - gt_depth
-    sel_d = mask & (hit != -1) & (gt_depth > 0) & (e < depth_error_max)
+    sel_d = mask & (hit != -1) & (gt_depth > 0) & ((e < depth_error_max) if depth_near is None else depth_near)
     nd = float(sel_d.sum())
     gcs = color_weight / (3 * n) if n > 0 else 0.0
     gds = depth_weight / nd if nd > 0 else 0.0
     cl = float(r.abs().sum()) / (3 * n) if n > 0 else 0.0
     dl = float(e[sel_d].abs().sum()) / nd if nd > 0 else 0.0
     sg = torch.sign(r)
-    return ((color_weight * cl + depth_weight * dl, cl, dl, nd), gcs * ea * sg, gds * torch.sign(e) * sel_d,
-            torch.tensor([gcs * float((sg * ea * render).sum()), gcs * float(sg.sum())], dtype=torch.float64))
+    nl, nn, gN = 0.0, 0.0, None
+    if normal is not None and normal_weight > 0:
+        sel_n = mask & (hit != -1) & (gt_normal != 0).any(0)
+        nn = float(sel_n.sum())
+        xl, yl = normal.norm(dim=0), gt_normal.norm(dim=0)
+        nx, ny = xl.clamp_min(1e-8), yl.clamp_min(1e-8)
+        cos = (normal * gt_normal).sum(0) / (nx * ny)
+        nl = float((1 - cos)[sel_n].sum()) / nn if nn > 0 else 0.0
+        gns = normal_weight / nn if nn > 0 else 0.0
+        # d cos / dx = y / (nx ny) - cos x / |x|^2 where |x| > 1e-8 (below, nx is the constant 1e-8)
+        dcos = gt_normal / (nx * ny) - torch.where(xl > 1e-8, cos / (nx * nx), torch.zeros_like(cos)) * normal
+        gN = -gns * dcos * sel_n
+    total = color_weight * cl + depth_weight * dl + (normal_weight * nl if gN is not None else 0.0)
+    return ([total, cl, dl, nd, nl, nn, 0.0, 0.0], gcs * ea * sg, gds * torch.sign(e) * sel_d, gN,
+            torch.tensor([gcs * float((sg * ea * render).sum()), gcs * float(sg.sum())], **f64))
 
 
 @pytest.mark.parametrize("ab", [(0.0, 0.0), (0.2, 0.05), (-0.25, -0.03)])
@@ -183,8 +205,8 @@ def test_l1_exposure_statement_matches_autograd(ab):
     gt_depth[::17] = 0.0
     hit = torch.where(torch.rand(n, generator=gen) < 0.9, 1, -1)
     mask = torch.rand(n, generator=gen) < 0.8
-    (loss, cl, dl, nd), gC, gD, gE = l1_exposure_statement(render.detach(), depth.detach(), hit, gt_color, gt_depth, mask, 0.8, 1.0,
-                                                          0.1, ab)
+    (loss, cl, dl, nd, *_), gC, gD, _, gE = loss_statement(render.detach(), depth.detach(), hit, gt_color, gt_depth, mask, 0.8, 1.0,
+                                                           0.1, ab)
     e = torch.tensor(ab, dtype=torch.float64, requires_grad=True)
     sel_d = mask & (hit != -1) & (gt_depth > 0) & ((depth.detach() - gt_depth) < 0.1)
     L = (0.8 * (torch.exp(e[0]) * render + e[1] - gt_color)[:, mask].abs().mean() + 1.0 * (depth - gt_depth)[sel_d].abs().mean())
@@ -192,6 +214,74 @@ def test_l1_exposure_statement_matches_autograd(ab):
     assert 0 < nd < n and abs(float(L.detach()) - loss) <= 1e-12 * loss
     assert float((aC - gC).abs().max()) <= 1e-15 and float((aD - gD).abs().max()) <= 1e-15
     assert float((aE - gE).abs().max()) <= 1e-12 * float(aE.abs().max())
+
+
+def mapping_frame(H, W, gen, dtype=torch.float64):
+    """A frame for the mapping loss as the loss tests build it: about half the depths within 0.1 of gt, 10 % of gt depths
+    0, 15 % of gt normals the zero vector and some with one or two zero components; render normals of length 0.5 - 1.5.
+    Returns render (3,H,W), depth (1,H,W), normal (3,H,W), depth_index (1,H,W) int32, gt_color (H,W,3), gt_depth (H,W,1),
+    gt_normal (H,W,3). `gen` is a torch.Generator; the tensors live on its device."""
+    import torch.nn.functional as F
+    kw = dict(generator=gen, device=gen.device)
+    u = lambda *s: torch.rand(*s, **kw)
+    render = u(3, H, W).to(dtype)
+    depth = (u(1, H, W) * 3).to(dtype)
+    normal = (F.normalize(torch.randn(3, H, W, **kw), dim=0) * (0.5 + u(1, H, W))).to(dtype)
+    depth_index = torch.randint(-1, 50, (1, H, W), dtype=torch.int32, **kw)
+    gt_color = u(H, W, 3).to(dtype)
+    near = depth.permute(1, 2, 0) + 0.05 * torch.randn(H, W, 1, **kw).to(dtype)
+    gt_depth = torch.where(u(H, W, 1) < 0.5, near, (u(H, W, 1) * 3).to(dtype))
+    gt_depth[u(H, W, 1) < 0.1] = 0
+    gt_normal = F.normalize(torch.randn(H, W, 3, **kw), dim=-1).to(dtype)
+    k = u(H, W)
+    gt_normal[k < 0.15] = 0
+    gt_normal[(k >= 0.15) & (k < 0.2), 0] = 0                                  # one zero component
+    gt_normal[(k >= 0.2) & (k < 0.25), 1:] = 0                                 # two zero components
+    return render, depth, normal, depth_index, gt_color, gt_depth, gt_normal
+
+
+@pytest.mark.parametrize("use_mask", [False, True])
+def test_loss_statement_is_the_mapping_loss_expressions(use_mask):
+    """The statement with the normal term against the eager expressions of Mapping.loss_update (mapper.py:402-451), as
+    test_mapping_loss_with_normal_and_ssim_terms writes them, differentiated by autograd in float64."""
+    import torch.nn.functional as F
+    H, W = 23, 31
+    gen = torch.Generator().manual_seed(11)
+    render, depth, normal, depth_index, gt_color, gt_depth, gt_normal = mapping_frame(H, W, gen)
+    mask = (torch.rand(H, W, generator=gen) < 0.6) if use_mask else None
+    for t in (render, depth, normal):
+        t.requires_grad_(True)
+    w = dict(color_weight=0.8, depth_weight=1.0, normal_weight=0.1)
+    image, d, nrm, di = render.permute(1, 2, 0), depth.permute(1, 2, 0), normal.permute(1, 2, 0), depth_index.permute(1, 2, 0)
+    rm = torch.ones(H, W, dtype=torch.bool) if mask is None else mask
+    color_loss = torch.abs(image[rm] - gt_color[rm]).mean()
+    err = d - gt_depth
+    valid = (di != -1).squeeze() & (gt_depth > 0).squeeze() & (err < 0.1).squeeze() & rm
+    depth_loss = torch.abs(err[valid]).mean()
+    cos_dist = 1 - F.cosine_similarity(nrm, gt_normal, dim=-1)
+    vn = rm & (di != -1).squeeze() & (~(gt_normal == 0).all(dim=-1))
+    normal_loss = cos_dist[vn].mean()
+    ref = w["depth_weight"] * depth_loss + w["normal_weight"] * normal_loss + w["color_weight"] * color_loss
+    aC, aD, aN = torch.autograd.grad(ref, (render, depth, normal))
+    n = H * W
+    parts, gC, gD, gN, gE = loss_statement(render.detach().reshape(3, n), depth.detach().reshape(n), depth_index.reshape(n),
+                                           gt_color.permute(2, 0, 1).reshape(3, n), gt_depth.reshape(n), rm.reshape(n), w["color_weight"],
+                                           w["depth_weight"], 0.1, normal=normal.detach().reshape(3, n),
+                                           gt_normal=gt_normal.permute(2, 0, 1).reshape(3, n), normal_weight=w["normal_weight"])
+    # the frame has every kind of pixel: a gt normal with one or two zero components takes part in the normal term
+    partial = (gt_normal == 0).any(-1) & ~(gt_normal == 0).all(-1)
+    assert 0 < parts[3] < n and 0 < parts[5] < n and int((vn & partial).sum()) > 0 and int((~vn & rm).sum()) > 0
+    assert parts[5] == int(vn.sum()) and parts[3] == int(valid.sum()) and parts[6:] == [0.0, 0.0]
+    for got, want in zip(parts[:3] + parts[4:5], (ref, color_loss, depth_loss, normal_loss)):
+        want = float(want.detach())
+        assert abs(got - want) <= 1e-13 * abs(want), (got, want)
+    for got, want in ((gC, aC), (gD, aD), (gN, aN)):
+        assert float((got.reshape(want.shape) - want).abs().max()) <= 1e-14 * float(want.abs().max())
+    # without the normal weight the statement is the L1 one: parts 4 and 5 are 0 and there is no normal gradient
+    p0, c0, d0, n0, _ = loss_statement(render.detach().reshape(3, n), depth.detach().reshape(n), depth_index.reshape(n),
+                                       gt_color.permute(2, 0, 1).reshape(3, n), gt_depth.reshape(n), rm.reshape(n), 0.8, 1.0, 0.1,
+                                       normal=normal.detach().reshape(3, n), gt_normal=gt_normal.permute(2, 0, 1).reshape(3, n))
+    assert n0 is None and p0[4:6] == [0.0, 0.0] and p0[1:4] == parts[1:4] and torch.equal(c0, gC) and torch.equal(d0, gD)
 
 
 # ------------------------------------------------------------------------------------------------------- the pyramid

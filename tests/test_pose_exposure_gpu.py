@@ -12,7 +12,7 @@ import torch
 
 from rtg_slam_b200 import scene
 from test_camera_grad_gpu import pose_error, se3_exp, view_camera
-from test_pose_exposure_cpu import exposure_gn_step, exposure_normal_equations, l1_exposure_statement
+from test_pose_exposure_cpu import exposure_gn_step, exposure_normal_equations, loss_statement
 from test_pose_gn_gpu import gn_inputs
 from test_pose_gn_pyramid_gpu import rows as plain_rows
 from test_pose_refine_cpu import camera_arrays
@@ -229,9 +229,9 @@ def test_loss_l1_exposure_matches_the_f64_statement(cuda_device, masks):
     # the selection from the float32 depth error, as the kernel forms it
     sel32 = (depth32 - gtd32) < torch.tensor(0.1, dtype=torch.float32)
     hit = torch.where(sel32, out["depth_index_map"].cpu().reshape(-1), torch.full((n,), -1, dtype=torch.int32))
-    (loss, cl, dl, nd), wC, wD, wE = l1_exposure_statement(out["render"].cpu().double().reshape(3, -1), depth32.double(), hit,
-                                                          tgt["render"].cpu().double().reshape(3, -1), gtd32.double(), m, 0.8, 1.0,
-                                                          float("inf"), ab32)
+    (loss, cl, dl, nd, *_), wC, wD, _, wE = loss_statement(out["render"].cpu().double().reshape(3, -1), depth32.double(), hit,
+                                                           tgt["render"].cpu().double().reshape(3, -1), gtd32.double(), m, 0.8, 1.0,
+                                                           float("inf"), ab32)
     assert nd > 0 and float(parts[3]) == nd
     for got, want in ((parts[0], loss), (parts[1], cl), (parts[2], dl)):
         assert abs(float(got) - want) <= 1e-6 * abs(want), (got, want)

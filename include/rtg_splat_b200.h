@@ -651,6 +651,32 @@ size_t rtg_knn_workspace_bytes(int64_t n_ref);
 int rtg_knn(const float *query, int64_t n_query, const float *ref, int64_t n_ref, int32_t K, int32_t skip_self, float *out_d2,
             int32_t *out_idx, float *out_mean, void *ws, void *stream);
 
+/* ---- the map follows corrected camera poses (no reference counterpart) --------------------------------------------
+ * rtg_map_transform: move every Gaussian rigidly with the correction of its anchor frame, in place. Anchor k has the
+ * camera-to-world poses old_c2w[k] and new_c2w[k] (K x 16 doubles, row-major 4x4, device). Once per anchor, in float64:
+ * q_delta = the unit quaternion (w >= 0) of R_new R_old^T, R = its rotation matrix, t = p_new - R p_old. Every row i with
+ * 0 <= anchor[i] < K whose anchor's two poses differ bitwise becomes
+ *   xyz' = R xyz + t,  rotation' = q_delta (x) rotation (Hamilton product, (w,x,y,z), the raw magnitude is kept),
+ *   normal' = R normal,  features_rest' band l = D^l(R) band l for l = 1..3 and each colour channel,
+ * where D^l is the rotation of band l of the rasterizer's real SH basis (computeColorFromSH, forward.cu:104-155):
+ * sh(f', R d) = sh(f, d) for every direction d. features_dc, scaling, opacity and every other attribute are untouched.
+ * Rows with anchor -1, or whose anchor's poses are bitwise equal, are not written; rows with any other anchor outside
+ * [0, K) are not written either and are counted in *n_skipped (device int64, set by the call). No host synchronisation.
+ * xyz (P,3), rotation (P,4), normal (P,3) or NULL, features_rest (P, sh_rest, 3) with sh_rest in {0, 3, 8, 15} (NULL iff
+ * sh_rest == 0), anchor (P) int32: device, fp32 / int32, contiguous. ws: rtg_map_transform_workspace_bytes(K) bytes,
+ * 16-byte aligned. P == 0: nothing is read and *n_skipped is set to 0. K == 0: no row is written, and *n_skipped counts
+ * every anchor other than -1 (old_c2w, new_c2w and ws may then be NULL). Validates on the host before any CUDA call: a
+ * NULL struct, a NULL required pointer, negative sizes and sh_rest outside the set are rejected. */
+typedef struct RtgMapTransform {
+    int32_t P, K, sh_rest, _pad;
+    const int32_t *anchor;                 /* (P) frame index per Gaussian (_add_tick), -1 = not anchored */
+    const double *old_c2w, *new_c2w;       /* (K,4,4) */
+    float *xyz, *rotation, *normal, *features_rest;
+    int64_t *n_skipped;                    /* rows whose anchor lies outside [-1, K) and != -1 */
+} RtgMapTransform;
+size_t rtg_map_transform_workspace_bytes(int32_t K);
+int rtg_map_transform(const RtgMapTransform *xf, void *ws, void *stream);
+
 /* ---- measurement hook (no reference counterpart) ---------------------------------------------
  * When enabled, every kernel launch of this library is bracketed by CUDA events on its launching stream.
  * rtg_profile_read synchronises the device and returns, per kernel id, the summed duration (ms) and the number

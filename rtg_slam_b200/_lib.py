@@ -90,6 +90,13 @@ class RtgPoseExposure(C.Structure):
     _fields_ = [("ab", C.c_void_p)]
 
 
+class RtgMapTransform(C.Structure):
+    """include/rtg_splat_b200.h: RtgMapTransform (field order is the ABI)."""
+    _fields_ = ([(n, C.c_int32) for n in ("P", "K", "sh_rest", "_pad")]
+                + [(n, C.c_void_p) for n in ("anchor", "old_c2w", "new_c2w", "xyz", "rotation", "normal", "features_rest",
+                                             "n_skipped")])
+
+
 class RtgIcpLevel(C.Structure):
     _fields_ = [("vertex0", C.c_void_p), ("normal0", C.c_void_p), ("vertex1", C.c_void_p), ("normal1", C.c_void_p),
                 ("H", C.c_int32), ("W", C.c_int32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
@@ -163,6 +170,8 @@ SIGNATURES = {
     "rtg_soa_compact": (C.c_int, [_VP, _I32, _I64, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "rtg_knn_workspace_bytes": (C.c_size_t, [_I64]),
     "rtg_knn": (C.c_int, [_VP, _I64, _VP, _I64, _I32, _I32, _VP, _VP, _VP, _VP, _VP]),
+    "rtg_map_transform_workspace_bytes": (C.c_size_t, [_I32]),
+    "rtg_map_transform": (C.c_int, [C.POINTER(RtgMapTransform), _VP, _VP]),
     "rtg_profile_enable": (C.c_int, [_I32]),
     "rtg_profile_kernel_count": (C.c_int, []),
     "rtg_profile_kernel_name": (C.c_char_p, [_I32]),

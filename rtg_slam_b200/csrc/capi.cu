@@ -1012,6 +1012,30 @@ int rtg_knn(const float *query, int64_t n_query, const float *ref, int64_t n_ref
     return check_launch("rtg_knn");
 }
 
+size_t rtg_map_transform_workspace_bytes(int32_t K) { return rtg::map_transform_ws_bytes(K); }
+
+int rtg_map_transform(const RtgMapTransform *xf, void *ws, void *stream) {
+    if (!xf) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_map_transform: xf is NULL");
+    if (xf->P < 0 || xf->K < 0) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_map_transform: bad sizes (P, K >= 0)");
+    if (xf->sh_rest != 0 && xf->sh_rest != 3 && xf->sh_rest != 8 && xf->sh_rest != 15)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_map_transform: sh_rest must be 0, 3, 8 or 15");
+    if (!xf->n_skipped) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_map_transform: NULL pointer (n_skipped)");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    if (xf->P == 0) {
+        cudaMemsetAsync(xf->n_skipped, 0, sizeof(int64_t), s);
+        return check_launch("rtg_map_transform");
+    }
+    if (!xf->anchor || !xf->xyz || !xf->rotation)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_map_transform: NULL pointer (anchor, xyz or rotation)");
+    if (xf->K > 0 && (!xf->old_c2w || !xf->new_c2w || !ws))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_map_transform: NULL pointer (old_c2w, new_c2w or ws)");
+    if ((xf->sh_rest == 0) != (xf->features_rest == nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_map_transform: features_rest must be NULL exactly when sh_rest == 0");
+    if (reinterpret_cast<uintptr_t>(ws) & 15) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_map_transform: ws must be 16-byte aligned");
+    rtg::launch_map_transform(*xf, ws, s);
+    return check_launch("rtg_map_transform");
+}
+
 int rtg_profile_enable(int32_t on) {
     std::lock_guard<std::mutex> lk(rtg::g_prof_mu);
     rtg::g_prof_on = on != 0;

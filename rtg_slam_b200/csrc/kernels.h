@@ -2,6 +2,8 @@
 #pragma once
 #include "common.cuh"
 
+struct RtgMapTransform;
+
 namespace rtg {
 
 void launch_preprocess_fwd(const ViewParams &vp, int P, int M, const float *means, const float *scales, const float *rots,
@@ -106,6 +108,10 @@ void launch_soa_compact(const uint8_t *mask, int invert, int64_t P, int n_arrays
 size_t knn_ws_bytes(int64_t n_ref);
 int launch_knn(const float *query, int64_t n_query, const float *ref, int64_t n_ref, int K, int skip_self, float *out_d2, int32_t *out_idx,
                float *out_mean, void *ws, cudaStream_t s);
+
+// maptransform.cu
+size_t map_transform_ws_bytes(int64_t K);
+void launch_map_transform(const RtgMapTransform &m, void *ws, cudaStream_t s);
 
 // adam.cu and the per-level icp.cu entry points are declared in their own sections of capi.cu
 }  // namespace rtg

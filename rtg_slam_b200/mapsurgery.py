@@ -11,7 +11,9 @@ Mirrors, with the reference's names, argument order and return values:
   `(dists (1,N,K) squared, idx (1,N,K) int64, knn (1,N,K,3) or None)`, neighbours sorted by distance;
 * `delete` / `remove` / `cat` of `GaussianPointCloud` (SLAM/gaussian_pointcloud.py:195-235,286-304) on a dict of the
   attribute tensors: one mask scan + one gather launch for all attributes and ONE host synchronisation (the new row
-  count) instead of one per attribute.
+  count) instead of one per attribute;
+* `transform(params, anchor, old_c2w, new_c2w)` (no reference counterpart): the map follows corrected camera poses --
+  every Gaussian moves rigidly, spherical harmonics included, with the correction of the frame that created it.
 
 Ties between equidistant neighbours may be reported with a different (equally near) index than the reference's
 Morton-box search or pytorch3d's would pick; distances are exact.
@@ -21,6 +23,7 @@ from __future__ import annotations
 import ctypes as C
 from collections import namedtuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -149,3 +152,91 @@ def remove(params: dict, remove_mask):
 def cat(params: dict, extra: dict):
     """GaussianPointCloud.cat for the attributes present in both dicts."""
     return {k: torch.cat([params[k], extra[k]]) if k in extra else params[k] for k in params}
+
+
+# ----------------------------------------------------------------------------- the map follows corrected poses
+SH_REST = (0, 3, 8, 15)
+
+
+def _poses(name, c2w):
+    """Host (K,4,4) camera-to-world poses as float64 numpy, checked to be rigid."""
+    if isinstance(c2w, torch.Tensor):
+        if c2w.is_cuda:
+            raise TypeError(f"{name} must be a host array (numpy or CPU tensor)")
+        c2w = c2w.detach().numpy()
+    a = np.ascontiguousarray(c2w, dtype=np.float64)
+    if a.ndim != 3 or a.shape[1:] != (4, 4):
+        raise ValueError(f"{name} must have shape (K, 4, 4), got {a.shape}")
+    if not np.isfinite(a).all():
+        raise ValueError(f"{name} has non-finite entries")
+    if not (a[:, 3] == np.array([0.0, 0.0, 0.0, 1.0])).all():
+        raise ValueError(f"{name}: the last row of every pose must be (0, 0, 0, 1)")
+    R = a[:, :3, :3]
+    if len(a) and (np.abs(R @ R.transpose(0, 2, 1) - np.eye(3)).max() > 1e-5 or (np.linalg.det(R) <= 0).any()):
+        raise ValueError(f"{name}: every rotation block must be orthonormal (to 1e-5) with det > 0")
+    return a
+
+
+def _rows(name, t, P, shape, dtype=torch.float32):
+    """`t` checked to be a contiguous CUDA (P, *shape) tensor of `dtype`; returned detached (same storage)."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dtype:
+        raise TypeError(f"{name} must be a CUDA {dtype} tensor")
+    if tuple(t.shape) != (P, *shape):
+        raise ValueError(f"{name} must have shape {(P, *shape)}, got {tuple(t.shape)}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous (it is updated in place)")
+    return t.detach()
+
+
+def transform(params: dict, anchor, old_c2w, new_c2w):
+    """Moves the map with corrected camera poses, in place: every Gaussian follows the correction
+    new_c2w[k] @ inv(old_c2w[k]) of its anchor frame k = anchor[i] (GaussianPointCloud._add_tick).
+
+    `params` holds the raw attribute tensors under the names of `remove()`: "xyz" (P,3) and "rotation" (P,4) are
+    required, "normal" (P,3) and "features_rest" (P,M-1,3), M in {1,4,9,16}, are moved when present (the spherical
+    harmonics are rotated band by band, so the rendered colour of a surfel does not change when it moves). Everything else
+    is left alone. anchor: (P,) or (P,1) int32 on the map's device; -1 = not anchored. old_c2w, new_c2w: host (K,4,4)
+    rigid camera-to-world poses (numpy or CPU tensors), validated here and uploaded without a synchronisation. Rows whose
+    anchor's two poses are equal are not written. Returns a device int64 tensor (1,): the number of rows whose anchor is
+    neither -1 nor in [0, K) (they are left unchanged; with K == 0 that is every anchored row); it is not read back."""
+    old, new = _poses("old_c2w", old_c2w), _poses("new_c2w", new_c2w)
+    if old.shape != new.shape:
+        raise ValueError(f"old_c2w and new_c2w differ in shape: {old.shape} vs {new.shape}")
+    xyz = params["xyz"]
+    if isinstance(xyz, torch.Tensor) and xyz.is_cuda and xyz.numel() == 0:  # an empty map (GaussianPointCloud's initial state)
+        return torch.zeros(1, dtype=torch.int64, device=xyz.device)
+    if not isinstance(xyz, torch.Tensor) or xyz.dim() != 2:
+        raise TypeError("params['xyz'] must be a (P, 3) CUDA float32 tensor")
+    P, K = xyz.shape[0], old.shape[0]
+    xyz = _rows("xyz", xyz, P, (3,))
+    dev = xyz.device
+    rot = _rows("rotation", params["rotation"], P, (4,))
+    normal = params.get("normal")
+    normal = None if normal is None else _rows("normal", normal, P, (3,))
+    rest = params.get("features_rest")
+    sh_rest = 0
+    if rest is not None:
+        if not isinstance(rest, torch.Tensor):
+            raise TypeError("features_rest must be a CUDA float32 tensor")
+        if rest.dim() != 3 or rest.shape[1] not in SH_REST:
+            raise ValueError("features_rest must be (P, M-1, 3) with M in {1, 4, 9, 16}")
+        sh_rest = rest.shape[1]
+        rest = _rows("features_rest", rest, P, (sh_rest, 3))
+    if not isinstance(anchor, torch.Tensor) or not anchor.is_cuda or anchor.dtype != torch.int32:
+        raise TypeError("anchor must be a CUDA int32 tensor")
+    if tuple(anchor.shape) not in ((P,), (P, 1)):
+        raise ValueError(f"anchor must have shape ({P},) or ({P}, 1), got {tuple(anchor.shape)}")
+    for name, t in (("rotation", rot), ("normal", normal), ("features_rest", rest), ("anchor", anchor)):
+        if t is not None and t.device != dev:
+            raise ValueError(f"{name} is not on the device of xyz")
+    anchor = anchor.contiguous()
+    poses = torch.from_numpy(np.stack([old, new])).pin_memory().to(dev, non_blocking=True)
+    n_skipped = torch.empty(1, dtype=torch.int64, device=dev)
+    L = _lib.lib()
+    ws = torch.empty(max(int(L.rtg_map_transform_workspace_bytes(K)), 16), dtype=torch.uint8, device=dev)
+    xf = _lib.RtgMapTransform(P=P, K=K, sh_rest=sh_rest, _pad=0, anchor=anchor.data_ptr(), old_c2w=poses[0].data_ptr(),
+                              new_c2w=poses[1].data_ptr(), xyz=xyz.data_ptr(), rotation=rot.data_ptr(),
+                              normal=None if normal is None else normal.data_ptr(),
+                              features_rest=None if sh_rest == 0 else rest.data_ptr(), n_skipped=n_skipped.data_ptr())
+    check(L.rtg_map_transform(C.byref(xf), _p(ws), _stream(dev)), "rtg_map_transform")
+    return n_skipped

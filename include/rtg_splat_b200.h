@@ -388,6 +388,25 @@ int rtg_splat_pose_gn_step_exposure(const RtgSplatView *view, int32_t P, int32_t
                                     int64_t R_cap, const int32_t *counters, const RtgPoseGN *s, const RtgPoseRobust *robust,
                                     const RtgPoseExposure *exposure, void *stream);
 
+/* ---- per-Gaussian contributions to a frame (no reference counterpart) ----------------------------------------------
+ * rtg_splat_contributions: what each Gaussian added to the render of one rtg_splat_forward (its view, workspaces, R_cap
+ * and counters; the view's flags must be the forward's). The pairs (p, g) that add colour are those the forward blends and
+ * the backward replays: p a pixel of a rendered tile, g at a position < n_contrib(p) of p's tile list, alpha past the
+ * 1/255 cut-off (the forward's decision, its recheck band included). Such a pair has the weight w(p, g) = alpha T, T the
+ * transmittance in front of g at p (the forward's colour weight). Per Gaussian g the call ADDS
+ *   n_pixels[g] += #{p : (p, g) adds colour}               (int32, at most H*W per call: exact),
+ *   weight[g]   += sum_p w(p, g),
+ *   error[g]    += sum_p w(p, g) pixel_error(p)           (only when pixel_error, (H, W) fp32 device, is given),
+ * so repeated calls sum over several frames. Culled Gaussians, masked-out and empty tiles and an overflowed forward
+ * (counters[RTG_CNT_OVERFLOW] != 0) add nothing. Summed over g, weight is sum_p (1 - T_map(p)) over the rendered pixels;
+ * error is the colour intermediate of rtg_splat_backward under dL/dcolor = (pixel_error, 0, 0). The float sums are
+ * accumulated with atomics in a varying order (not bit-reproducible); the counts are. No Gaussian parameter array is read.
+ * n_pixels, weight, error: P rows, device, 4-byte aligned; n_pixels and weight are required when P > 0; error and
+ * pixel_error are both NULL or both given. Validates on the host before any CUDA work; P == 0 does no work. */
+int rtg_splat_contributions(const RtgSplatView *view, int32_t P, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                            int64_t R_cap, const int32_t *counters, const float *pixel_error, int32_t *n_pixels, float *weight,
+                            float *error, void *stream);
+
 /* Replaces CudaRasterizer::Rasterizer::markVisible (rasterizer.h:21-26, rasterizer_impl.cu:145-157). */
 int rtg_splat_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix,
                            uint8_t *present, void *stream);

@@ -133,6 +133,8 @@ SIGNATURES = {
     "rtg_splat_pose_gn_scratch_bytes": (C.c_size_t, [_I32, _I32, _I32]),
     # view, P, M, 6 Gaussian inputs, 3 workspaces, R_cap, counters, then hit_image, scratch, J / the step's state, stream
     "rtg_splat_pose_tangents": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP] + [_VP] * 4),
+    # view, P, the three workspaces, R_cap, counters, pixel_error, n_pixels, weight, error, stream
+    "rtg_splat_contributions": (C.c_int, [C.POINTER(RtgSplatView), _I32] + [_VP] * 3 + [_I64, _VP] + [_VP] * 4 + [_VP]),
     "rtg_splat_pose_gn_step": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
                                + [C.POINTER(RtgPoseGN), _VP]),
     "rtg_splat_pose_gn_step_robust": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]

@@ -580,6 +580,32 @@ int rtg_splat_pose_tangents(const RtgSplatView *view, int32_t P, int32_t M, cons
     return check_launch(who);
 }
 
+int rtg_splat_contributions(const RtgSplatView *view, int32_t P, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                            int64_t R_cap, const int32_t *counters, const float *pixel_error, int32_t *n_pixels, float *weight,
+                            float *error, void *stream) {
+    const char *who = "rtg_splat_contributions";
+    int rc = validate_view(view, who);
+    if (rc) return rc;
+    if (P < 0) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": P < 0");
+    if (R_cap < 0) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": R_cap < 0");
+    if (!geom_ws || !img_ws || !bin_ws || !counters)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL workspace / counters");
+    if (P > 0 && (!n_pixels || !weight)) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL n_pixels / weight");
+    if ((error == nullptr) != (pixel_error == nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": error and pixel_error must be given together");
+    if ((((uintptr_t)n_pixels) | ((uintptr_t)weight) | ((uintptr_t)error) | ((uintptr_t)pixel_error)) & 3)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": outputs / pixel_error must be 4-byte aligned");
+    if (P == 0) return RTG_OK;  // no Gaussian, no tile list entry
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const rtg::ViewParams vp = make_view(view);
+    const int T = vp.tiles_x * vp.tiles_y;
+    rtg::GeomState g = rtg::geom_from(const_cast<void *>(geom_ws), (size_t)P);
+    rtg::ImgState img = rtg::img_from(const_cast<void *>(img_ws), (size_t)vp.H * vp.W);
+    rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
+    rtg::launch_render_contributions(vp, g, b, img, counters, pixel_error, n_pixels, weight, error, s);
+    return check_launch(who);
+}
+
 // The step of the Gauss-Newton entry points: `robust` selects the normal-equation rows (RTG_ROBUST_NONE: the plain ones),
 // `ab` (the device exposure, or nullptr) the eight-unknown step.
 static int pose_gn_step(const char *who, const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,

@@ -1284,4 +1284,111 @@ void launch_render_bwd(const ViewParams &vp, const GeomState &g, const BinState 
         render_bwd_kernel<false><<<T, BWD_THREADS, 0, s>>>(vp, g, b, img, counters, final_T, hit_image, dL_dcolor, dL_ddepth, rec, nullptr);
 }
 
+// ------------------------------------------------------------------ per-Gaussian contributions
+// What each Gaussian adds to the forward's render, replayed from the forward's own decisions as in render_tangent_body:
+// one CTA per tile in the forward's launch order, one pixel per thread on the forward's 8x4 warp patches, the tile's list
+// walked front to back up to its longest blended prefix with the same patch masks, pretest and alpha function and a
+// pixel's own n_contrib. A pixel carries only T: every pair it blends has the forward's colour weight w = alpha T, then
+// T *= 1 - alpha, bit for bit as render_fwd_kernel. Per (warp, entry) with at least one blending lane, the count of those
+// lanes goes to n_pixels and the warp sums of w (and, ERR, of w e with e the pixel's error) go to weight (and error):
+// one butterfly for both sums (after the xor-16 step lanes 0-15 hold w, lanes 16-31 w e), lane 0 adds the count and
+// sum w, lane 16 sum w e. The atomics' results are unused (RED). Reads no parameter array and no colour.
+template <bool ERR>
+__global__ void __launch_bounds__(256) render_contrib_kernel(const ViewParams vp, const GeomState g, const BinState b, const ImgState img,
+                                                             const int *__restrict__ counters, const float *__restrict__ pixel_error,
+                                                             int *__restrict__ n_pixels, float *__restrict__ weight,
+                                                             float *__restrict__ error) {
+    __shared__ float4 s_s0[BATCH], s_s1[BATCH];
+    __shared__ int s_id[BATCH];
+    __shared__ uint32_t s_mask[BATCH];
+    __shared__ uint32_t s_max[8];
+
+    if (counters[2] != 0) return;  // an overflowed forward rendered nothing
+    const int tile = (int)b.active[blockIdx.x];
+    const int n = (int)b.tile_count[(size_t)tile * RTG_CNT_STRIDE];
+    if (n == 0) return;            // empty or masked-out tile
+    int px, py;
+    bool inside;
+    pixel_of(vp, tile, px, py, inside);
+    const int pix = vp.W * py + px;
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const uint32_t start = b.tile_offset[tile];
+    const uint32_t last = inside ? img.n_contrib[pix] : 0u;
+    float e = 0.f;
+    if constexpr (ERR) e = inside ? pixel_error[pix] : 0.f;
+    uint32_t wmax = last;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(FULL, wmax, o));
+    if (lane == 0) s_max[w] = wmax;
+    __syncthreads();
+    uint32_t m = 0;
+#pragma unroll
+    for (int k = 0; k < 8; k++) m = max(m, s_max[k]);
+
+    const float pxf = (float)px, pyf = (float)py;
+    const float tx0 = (float)((tile % vp.tiles_x) * RTG_TILE), ty0 = (float)((tile / vp.tiles_x) * RTG_TILE);
+    float T = 1.f;
+    const int rounds = ((int)m + BATCH - 1) / BATCH;
+    for (int i = 0; i < rounds; i++) {
+        __syncthreads();  // the previous round has been consumed
+        if (i * BATCH + (int)threadIdx.x < (int)m) {
+            const int id = (int)b.point_list[start + (size_t)i * BATCH + threadIdx.x];
+            const float4 s0 = __ldg(g.splat + 2 * (size_t)id), s1 = __ldg(g.splat + 2 * (size_t)id + 1);
+            s_id[threadIdx.x] = id;
+            s_s0[threadIdx.x] = s0;
+            s_s1[threadIdx.x] = s1;
+            s_mask[threadIdx.x] = patch_mask(s0, s1, tx0, ty0);
+        }
+        __syncthreads();
+        const int cnt = min(BATCH, (int)m - i * BATCH);
+        for (int c = 0; c < ((cnt + 31) >> 5); c++) {
+            const int ej = (c << 5) + lane;
+            const uint32_t mm = ej < cnt ? s_mask[ej] : 0u;
+            uint32_t bits = __ballot_sync(FULL, (mm >> w) & 1u);
+            while (bits) {
+                const int j = (c << 5) + __ffs(bits) - 1;
+                bits &= bits - 1;
+                const uint32_t pos = (uint32_t)(i * BATCH + j);
+                const float4 s0 = s_s0[j], s1 = s_s1[j];
+                const float power = pair_power(s1.x, s1.y, s1.z, s0.x - pxf, s0.y - pyf);
+                float alpha, au;
+                const bool ok = pos < last && RTG_FWD_PRETEST(power, s0.z) && pair_alpha(power, s1.w, s0.w, alpha, au);
+                const uint32_t who = __ballot_sync(FULL, ok);
+                if (who == 0u) continue;
+                float wt = 0.f;
+                if (ok) {
+                    wt = alpha * T;
+                    T = T * (1.f - alpha);
+                }
+                float v;
+                if constexpr (ERR) {
+                    const float we = ok ? wt * e : 0.f;
+                    const bool hi = lane & 16;
+                    v = (hi ? we : wt) + __shfl_xor_sync(FULL, hi ? wt : we, 16);
+                } else {
+                    v = wt + __shfl_xor_sync(FULL, wt, 16);
+                }
+#pragma unroll
+                for (int o = 8; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+                if (lane == 0) {
+                    const int id = s_id[j];
+                    atomicAdd(n_pixels + id, __popc(who));
+                    atomicAdd(weight + id, v);
+                }
+                if (ERR && lane == 16) atomicAdd(error + s_id[j], v);
+            }
+        }
+    }
+}
+
+void launch_render_contributions(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                                 const int32_t *counters, const float *pixel_error, int32_t *n_pixels, float *weight, float *error,
+                                 cudaStream_t s) {
+    const int T = vp.tiles_x * vp.tiles_y;
+    if (pixel_error)
+        render_contrib_kernel<true><<<T, 256, 0, s>>>(vp, g, b, img, counters, pixel_error, n_pixels, weight, error);
+    else
+        render_contrib_kernel<false><<<T, 256, 0, s>>>(vp, g, b, img, counters, nullptr, n_pixels, weight, nullptr);
+}
+
 }  // namespace rtg

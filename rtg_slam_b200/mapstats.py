@@ -6,7 +6,7 @@ Same names and argument meaning as the reference:
 * `pixelmask2tilemask`, `transmission2tilemask`, `colorerror2tilemask` -- SLAM/utils.py:681-734, called by
   Mapping.evaluate_render_range (mapper.py:471-508);
 plus two fused entry points for that caller: `transmission_masks(T_map)` = (render_mask, tile_mask) in one pass and
-`color_error_map(render, gt)`.
+`color_error_map(render, gt)`, and `gaussian_contributions`, what every Gaussian adds to a frame (rtg_splat_contributions).
 """
 from __future__ import annotations
 
@@ -14,7 +14,7 @@ import ctypes as C
 
 import torch
 
-from . import _lib
+from . import _lib, rasterizer
 from ._lib import check
 
 
@@ -119,3 +119,53 @@ def color_error_map(render, gt):
     out = torch.empty((H, W), dtype=torch.float32, device=r.device)
     check(_lib.lib().rtg_color_error(H, W, _p(r), _p(g), _p(out), _stream(r.device)), "rtg_color_error")
     return out
+
+
+def gaussian_contributions(raster_settings, means3D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
+                           cov3D_precomp=None, tile_mask=None, pixel_error=None, out=None):
+    """One rasterizer forward and what each Gaussian added to it (rtg_splat_contributions). A pair (pixel p, Gaussian g)
+    adds colour when the forward blends it; its weight is w = alpha T, the forward's colour weight. Per Gaussian:
+      n_pixels (int32)  the pixels g adds colour to,
+      weight (float32)  sum_p w(p, g)  (an importance score; sum_g = sum_p (1 - T_map) over the rendered pixels),
+      error (float32)   sum_p w(p, g) pixel_error(p), only with `pixel_error` (H, W) float32: every pixel's error shared
+                        among all the Gaussians that blend into it, not only the arg-max of accumulate_gaussian_error.
+    Inputs as GaussianRasterizer takes them; the mode of `rasterizer.antialiased()` applies. A forward that overflows its
+    binning buffer is rendered again once; a second overflow raises CapacityOverflow. `out`: a dict of such (P,) CUDA
+    tensors to add into (for sums over several frames); without it zeroed tensors are allocated.
+    Returns (outputs, stats): the forward's eight outputs as GaussianRasterizer returns them and the dict. Nothing is
+    differentiated by autograd."""
+    with torch.no_grad():
+        dev = means3D.device
+        st = rasterizer._state(dev)
+        P = int(means3D.shape[0])
+        H, W = int(raster_settings.image_height), int(raster_settings.image_width)
+        pe = None if pixel_error is None else _f32("pixel_error", pixel_error, H * W)
+        if pe is not None and pe.device != dev:
+            raise ValueError(f"pixel_error is on {pe.device}, expected {dev}")
+        want = {"n_pixels": torch.int32, "weight": torch.float32}
+        if pe is not None:
+            want["error"] = torch.float32
+        if out is None:
+            stats = {k: torch.zeros((P,), dtype=dt, device=dev) for k, dt in want.items()}
+        else:
+            if set(out) != set(want):
+                raise ValueError(f"out must hold exactly {sorted(want)}")
+            for k, dt in want.items():
+                t = out[k]
+                if not torch.is_tensor(t) or t.dtype != dt or t.device != dev or tuple(t.shape) != (P,) or not t.is_contiguous():
+                    raise ValueError(f"out[{k!r}] must be a contiguous ({P},) {dt} tensor on {dev}")
+            stats = out
+        for attempt in range(2):
+            outs, saved, _ = rasterizer._forward_native(raster_settings, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                                        cov3D_precomp, tile_mask)
+            st.read(saved.pending, block=True)
+            if not saved.pending.overflow:
+                break
+            if attempt:
+                raise rasterizer.CapacityOverflow("gaussian_contributions: the render overflowed the binning buffer twice")
+        view, keep = rasterizer._make_view(raster_settings, dev, saved.antialiased)
+        check(_lib.lib().rtg_splat_contributions(C.byref(view), P, C.c_void_p(saved.geom), C.c_void_p(saved.img),
+                                                 C.c_void_p(saved.bin), saved.r_cap, C.c_void_p(saved.counters), _p(pe),
+                                                 _p(stats["n_pixels"]), _p(stats["weight"]), _p(stats.get("error")), _stream(dev)),
+              "rtg_splat_contributions")
+        return outs, stats

@@ -407,6 +407,27 @@ int rtg_splat_contributions(const RtgSplatView *view, int32_t P, const void *geo
                             int64_t R_cap, const int32_t *counters, const float *pixel_error, int32_t *n_pixels, float *weight,
                             float *error, void *stream);
 
+/* ---- per-Gaussian feature maps (no reference counterpart) ---------------------------------------------------------
+ * rtg_splat_features: a C-channel image of per-Gaussian features composited with the blend weights of one
+ * rtg_splat_forward (its view, workspaces, R_cap and counters; the view's flags must be the forward's). With w(p, g) =
+ * alpha T, the forward's colour weight of the pairs it blends (as in rtg_splat_contributions),
+ *   out[c, p] = sum_g w(p, g) features[g, c]        features (P, C) row-major, out (C, H, W), both fp32 device.
+ * Every pixel of out is written: 0 on masked-out and empty tiles and everywhere when the forward overflowed
+ * (counters[RTG_CNT_OVERFLOW] != 0). There is no background term (T_map is the remainder). With features = the forward's
+ * colours this is its colour image without the background; with features = 1 it is 1 - T_map.
+ * rtg_splat_features_backward: the transpose with the weights held fixed,
+ *   dL_dfeatures[g, c] = sum_p w(p, g) dL_dout[c, p]   dL_dout (C, H, W), dL_dfeatures (P, C), overwritten.
+ * Rows the frame never blends (culled Gaussians among them) are 0, and so is every row after an overflowed forward. The
+ * sums are accumulated with atomics in a varying order (not bit-reproducible); the forward map is. No Gaussian parameter
+ * array is read. 1 <= C <= RTG_FEATURES_MAX. Both validate on the host before any CUDA work; with P == 0 the forward only
+ * zeroes out and the backward does nothing. */
+enum { RTG_FEATURES_MAX = 128 };
+int rtg_splat_features(const RtgSplatView *view, int32_t P, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                       int64_t R_cap, const int32_t *counters, int32_t C, const float *features, float *out, void *stream);
+int rtg_splat_features_backward(const RtgSplatView *view, int32_t P, const void *geom_ws, const void *img_ws,
+                                const void *bin_ws, int64_t R_cap, const int32_t *counters, int32_t C, const float *dL_dout,
+                                float *dL_dfeatures, void *stream);
+
 /* Replaces CudaRasterizer::Rasterizer::markVisible (rasterizer.h:21-26, rasterizer_impl.cu:145-157). */
 int rtg_splat_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix,
                            uint8_t *present, void *stream);

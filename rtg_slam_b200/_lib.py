@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get("RTG_SPLAT_LIB") or os.path.join(HERE, "librtg_splat_b
 
 RTG_CNT_WORDS = 8
 RTG_ADAM_MAX_GROUPS = 8
+RTG_FEATURES_MAX = 128  # channels of rtg_splat_features
 # bits of RtgSplatView.prefiltered (a flags word)
 RTG_VIEW_PREFILTERED, RTG_VIEW_ANTIALIASED = 1, 2
 
@@ -135,6 +136,9 @@ SIGNATURES = {
     "rtg_splat_pose_tangents": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP] + [_VP] * 4),
     # view, P, the three workspaces, R_cap, counters, pixel_error, n_pixels, weight, error, stream
     "rtg_splat_contributions": (C.c_int, [C.POINTER(RtgSplatView), _I32] + [_VP] * 3 + [_I64, _VP] + [_VP] * 4 + [_VP]),
+    # view, P, the three workspaces, R_cap, counters, C, input (features / dL_dout), output, stream
+    "rtg_splat_features": (C.c_int, [C.POINTER(RtgSplatView), _I32] + [_VP] * 3 + [_I64, _VP, _I32] + [_VP] * 3),
+    "rtg_splat_features_backward": (C.c_int, [C.POINTER(RtgSplatView), _I32] + [_VP] * 3 + [_I64, _VP, _I32] + [_VP] * 3),
     "rtg_splat_pose_gn_step": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
                                + [C.POINTER(RtgPoseGN), _VP]),
     "rtg_splat_pose_gn_step_robust": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]

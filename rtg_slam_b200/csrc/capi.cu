@@ -606,6 +606,66 @@ int rtg_splat_contributions(const RtgSplatView *view, int32_t P, const void *geo
     return check_launch(who);
 }
 
+// The checks the two feature entry points share; `in` is the (P, C) features or the (C, H, W) upstream gradient, `out` the
+// other one.
+static int validate_features(const char *who, const RtgSplatView *view, int32_t P, const void *geom_ws, const void *img_ws,
+                             const void *bin_ws, int64_t R_cap, const int32_t *counters, int32_t C, const float *in,
+                             const float *out, bool out_needed) {
+    int rc = validate_view(view, who);
+    if (rc) return rc;
+    if (P < 0) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": P < 0");
+    if (R_cap < 0) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": R_cap < 0");
+    if (C < 1 || C > RTG_FEATURES_MAX)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": C must be 1.." + std::to_string(RTG_FEATURES_MAX) +
+                                                  ", got " + std::to_string(C));
+    if (P > 0 && (!geom_ws || !img_ws || !bin_ws || !counters))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL workspace / counters");
+    if ((P > 0 || out_needed) && !out) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL output");
+    if (P > 0 && !in) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL input");
+    if ((((uintptr_t)in) | ((uintptr_t)out)) & 3)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": input / output must be 4-byte aligned");
+    return RTG_OK;
+}
+
+int rtg_splat_features(const RtgSplatView *view, int32_t P, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                       int64_t R_cap, const int32_t *counters, int32_t C, const float *features, float *out, void *stream) {
+    const char *who = "rtg_splat_features";
+    int rc = validate_features(who, view, P, geom_ws, img_ws, bin_ws, R_cap, counters, C, features, out, true);
+    if (rc) return rc;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const rtg::ViewParams vp = make_view(view);
+    if (P == 0) {  // no Gaussian: an empty map
+        cudaError_t e = cudaMemsetAsync(out, 0, (size_t)C * vp.H * vp.W * sizeof(float), s);
+        if (e != cudaSuccess) return fail(RTG_ERR_CUDA, std::string(who) + " memset: " + cudaGetErrorString(e));
+        return RTG_OK;
+    }
+    const int T = vp.tiles_x * vp.tiles_y;
+    rtg::GeomState g = rtg::geom_from(const_cast<void *>(geom_ws), (size_t)P);
+    rtg::ImgState img = rtg::img_from(const_cast<void *>(img_ws), (size_t)vp.H * vp.W);
+    rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
+    rtg::launch_render_features(vp, g, b, img, counters, C, features, out, s);
+    return check_launch(who);
+}
+
+int rtg_splat_features_backward(const RtgSplatView *view, int32_t P, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                                int64_t R_cap, const int32_t *counters, int32_t C, const float *dL_dout, float *dL_dfeatures,
+                                void *stream) {
+    const char *who = "rtg_splat_features_backward";
+    int rc = validate_features(who, view, P, geom_ws, img_ws, bin_ws, R_cap, counters, C, dL_dout, dL_dfeatures, false);
+    if (rc) return rc;
+    if (P == 0) return RTG_OK;  // no row to write
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const rtg::ViewParams vp = make_view(view);
+    cudaError_t e = cudaMemsetAsync(dL_dfeatures, 0, (size_t)P * C * sizeof(float), s);  // rows the frame never blends
+    if (e != cudaSuccess) return fail(RTG_ERR_CUDA, std::string(who) + " memset: " + cudaGetErrorString(e));
+    const int T = vp.tiles_x * vp.tiles_y;
+    rtg::GeomState g = rtg::geom_from(const_cast<void *>(geom_ws), (size_t)P);
+    rtg::ImgState img = rtg::img_from(const_cast<void *>(img_ws), (size_t)vp.H * vp.W);
+    rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
+    rtg::launch_render_features_bwd(vp, g, b, img, counters, C, dL_dout, dL_dfeatures, s);
+    return check_launch(who);
+}
+
 // The step of the Gauss-Newton entry points: `robust` selects the normal-equation rows (RTG_ROBUST_NONE: the plain ones),
 // `ab` (the device exposure, or nullptr) the eight-unknown step.
 static int pose_gn_step(const char *who, const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,

@@ -60,6 +60,12 @@ void launch_render_tangent_images(const ViewParams &vp, int P, const GeomState &
 void launch_render_contributions(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
                                  const int32_t *counters, const float *pixel_error, int32_t *n_pixels, float *weight, float *error,
                                  cudaStream_t s);
+// the forward's blend weights applied to C per-Gaussian features: out (C, H, W) written everywhere; and its transpose,
+// dL_dfeatures (P, C) added into (the caller zeroes it)
+void launch_render_features(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                            const int32_t *counters, int C, const float *features, float *out, cudaStream_t s);
+void launch_render_features_bwd(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                                const int32_t *counters, int C, const float *dL_dout, float *dL_dfeatures, cudaStream_t s);
 
 // mapstats.cu
 void launch_gs_error(int H, int W, int P, const float *color_err, const float *depth_err, const float *normal_err,

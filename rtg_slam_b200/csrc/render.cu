@@ -1391,4 +1391,237 @@ void launch_render_contributions(const ViewParams &vp, const GeomState &g, const
         render_contrib_kernel<false><<<T, 256, 0, s>>>(vp, g, b, img, counters, nullptr, n_pixels, weight, nullptr);
 }
 
+// ------------------------------------------------------------------ per-Gaussian feature maps
+// out[c, p] = sum_g w(p, g) F[g, c] and its transpose dL/dF[g, c] = sum_p w(p, g) G[c, p], with w = alpha T the forward's
+// colour weight, replayed as render_contrib_kernel replays it. A CTA renders K channels [c0, c0 + K) of one tile; CTA
+// b takes tile active[b / chunks] and chunk b % chunks, so the chunks of a heavy tile start together, early.
+
+// Shared memory of one replay: the staged batch's splat records, ids and patch masks, and the warps' longest prefixes.
+struct ReplaySmem {
+    float4 s0[BATCH], s1[BATCH];
+    int id[BATCH];
+    uint32_t mask[BATCH];
+    uint32_t wmax[8];
+};
+
+// The forward's colour blending of one tile, replayed front to back up to the longest prefix its pixels blended (max
+// n_contrib), with the forward's patch masks, pretest and alpha function and the pixel's own n_contrib (`last`; 0 outside
+// the image). Every thread of the CTA must call it. stage(slot, id) runs once per staged entry on its staging thread
+// (before the batch's barrier); visit(slot, ok, wt) runs for every (warp, entry) the warp's patch mask lets through,
+// warp-uniformly, with ok = the pair blends and wt = alpha T (0 when !ok); T then advances bit for bit as in
+// render_fwd_kernel. Returns the pixel's final T.
+template <typename Stage, typename Visit>
+__device__ __forceinline__ float replay_blends(const ViewParams &vp, const GeomState &g, const BinState &b, const int tile,
+                                               const uint32_t last, const float pxf, const float pyf, ReplaySmem &sm,
+                                               Stage stage, Visit visit) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const uint32_t start = b.tile_offset[tile];
+    uint32_t wmax = last;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(FULL, wmax, o));
+    if (lane == 0) sm.wmax[w] = wmax;
+    __syncthreads();
+    uint32_t m = 0;
+#pragma unroll
+    for (int k = 0; k < 8; k++) m = max(m, sm.wmax[k]);
+
+    const float tx0 = (float)((tile % vp.tiles_x) * RTG_TILE), ty0 = (float)((tile / vp.tiles_x) * RTG_TILE);
+    float T = 1.f;
+    const int rounds = ((int)m + BATCH - 1) / BATCH;
+    for (int i = 0; i < rounds; i++) {
+        __syncthreads();  // the previous round has been consumed
+        if (i * BATCH + (int)threadIdx.x < (int)m) {
+            const int id = (int)b.point_list[start + (size_t)i * BATCH + threadIdx.x];
+            const float4 s0 = __ldg(g.splat + 2 * (size_t)id), s1 = __ldg(g.splat + 2 * (size_t)id + 1);
+            sm.id[threadIdx.x] = id;
+            sm.s0[threadIdx.x] = s0;
+            sm.s1[threadIdx.x] = s1;
+            sm.mask[threadIdx.x] = patch_mask(s0, s1, tx0, ty0);
+            stage((int)threadIdx.x, id);
+        }
+        __syncthreads();
+        const int cnt = min(BATCH, (int)m - i * BATCH);
+        for (int c = 0; c < ((cnt + 31) >> 5); c++) {
+            const int ej = (c << 5) + lane;
+            const uint32_t mm = ej < cnt ? sm.mask[ej] : 0u;
+            uint32_t bits = __ballot_sync(FULL, (mm >> w) & 1u);
+            while (bits) {
+                const int j = (c << 5) + __ffs(bits) - 1;
+                bits &= bits - 1;
+                const uint32_t pos = (uint32_t)(i * BATCH + j);
+                const float4 s0 = sm.s0[j], s1 = sm.s1[j];
+                const float power = pair_power(s1.x, s1.y, s1.z, s0.x - pxf, s0.y - pyf);
+                float alpha, au;
+                const bool ok = pos < last && RTG_FWD_PRETEST(power, s0.z) && pair_alpha(power, s1.w, s0.w, alpha, au);
+                float wt = 0.f;
+                if (ok) {
+                    wt = alpha * T;
+                    T = T * (1.f - alpha);
+                }
+                visit(j, ok, wt);
+            }
+        }
+    }
+    return T;
+}
+
+// Row stride (floats) of a staged feature chunk: 16-byte rows whose quarter-warp STS.128 fall into distinct banks.
+template <int K>
+constexpr int feat_stride() { return K == 4 ? 4 : K + 4; }
+
+// Forward: each pixel keeps K accumulators; each staged entry's K features of the chunk sit in shared memory next to its
+// splat record (channels >= C staged as 0). Every pixel of the image is written: 0 where the tile is empty, masked out or
+// the forward overflowed (no background term: T_map holds the remainder).
+template <int K>
+__global__ void __launch_bounds__(256) render_feat_fwd_kernel(const ViewParams vp, const GeomState g, const BinState b,
+                                                              const ImgState img, const int *__restrict__ counters,
+                                                              const int C, const int chunks, const float *__restrict__ F,
+                                                              float *__restrict__ out) {
+    constexpr int FS = feat_stride<K>();
+    __shared__ ReplaySmem sm;
+    __shared__ __align__(16) float s_f[BATCH * FS];
+
+    const int tile = (int)b.active[blockIdx.x / chunks];
+    const int c0 = (int)(blockIdx.x % chunks) * K;
+    const int kc = min(K, C - c0);
+    int px, py;
+    bool inside;
+    pixel_of(vp, tile, px, py, inside);
+    const int pix = vp.W * py + px;
+    const size_t N = (size_t)vp.H * vp.W;
+    float acc[K];
+#pragma unroll
+    for (int k = 0; k < K; k++) acc[k] = 0.f;
+    const int n = counters[2] != 0 ? 0 : (int)b.tile_count[(size_t)tile * RTG_CNT_STRIDE];
+    if (n > 0) {  // block-uniform
+        const uint32_t last = inside ? img.n_contrib[pix] : 0u;
+        auto stage = [&](const int slot, const int id) {
+            const float *row = F + (size_t)id * C + c0;
+            float v[K];
+#pragma unroll
+            for (int k = 0; k < K; k++) v[k] = k < kc ? __ldg(row + k) : 0.f;
+            float4 *dst = reinterpret_cast<float4 *>(s_f + slot * FS);
+#pragma unroll
+            for (int q = 0; q < K / 4; q++) dst[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+        };
+        auto visit = [&](const int j, const bool ok, const float wt) {
+            if (!ok) return;
+            const float4 *row = reinterpret_cast<const float4 *>(s_f + j * FS);
+#pragma unroll
+            for (int q = 0; q < K / 4; q++) {
+                const float4 f = row[q];
+                acc[4 * q] += wt * f.x;
+                acc[4 * q + 1] += wt * f.y;
+                acc[4 * q + 2] += wt * f.z;
+                acc[4 * q + 3] += wt * f.w;
+            }
+        };
+        replay_blends(vp, g, b, tile, last, (float)px, (float)py, sm, stage, visit);
+    }
+    if (inside) {
+#pragma unroll
+        for (int k = 0; k < K; k++)
+            if (k < kc) out[(size_t)(c0 + k) * N + pix] = acc[k];
+    }
+}
+
+template <int K>
+constexpr int feat_log2() { return K == 16 ? 4 : (K == 8 ? 3 : 2); }
+
+// Sum K per-lane values (K a power of two, 4..16) across the warp by recursive halving: at the step xor o (o = 16, 8, ...)
+// a lane keeps one half of its values, the upper half if lane & o, and adds its partner's copy of that half (K/2, K/4, ...
+// shuffles); once one value is left the remaining steps are plain butterfly adds. K - 1 + 5 - log2(K) shuffles in all
+// (16 for K = 16, instead of 5 K). Afterwards lane l holds the total of value l >> (5 - log2 K) (feat_slot).
+template <int K>
+__device__ __forceinline__ float warp_reduce_halving(float v[K], const int lane) {
+#pragma unroll
+    for (int step = 0; step < feat_log2<K>(); step++) {
+        const int h = K >> (step + 1), o = 16 >> step;
+        // the halves are swapped with a bit mask, not a select: a select of two array elements becomes a select of their
+        // addresses, which puts v in local memory
+        const uint32_t hm = (lane & o) ? FULL : 0u;
+#pragma unroll
+        for (int k = 0; k < h; k++) {
+            const uint32_t lo_bits = __float_as_uint(v[k]), hi_bits = __float_as_uint(v[h + k]);
+            const float keep = __uint_as_float((hi_bits & hm) | (lo_bits & ~hm));
+            const float send = __uint_as_float((lo_bits & hm) | (hi_bits & ~hm));
+            v[k] = keep + __shfl_xor_sync(FULL, send, o);
+        }
+    }
+    float s = v[0];
+#pragma unroll
+    for (int o = 32 / (2 * K); o > 0; o >>= 1) s += __shfl_xor_sync(FULL, s, o);
+    return s;
+}
+
+// Backward: each pixel holds its K upstream values; per (warp, entry) with at least one blending lane the warp sums w G[c]
+// of the K channels with warp_reduce_halving and adds them with one RED per channel, issued together by K lanes (K
+// consecutive floats of the row). dL_dF must be zeroed by the caller: rows the frame never blends are left alone.
+template <int K>
+__global__ void __launch_bounds__(256) render_feat_bwd_kernel(const ViewParams vp, const GeomState g, const BinState b,
+                                                              const ImgState img, const int *__restrict__ counters,
+                                                              const int C, const int chunks, const float *__restrict__ dL_dout,
+                                                              float *__restrict__ dL_dF) {
+    __shared__ ReplaySmem sm;
+
+    if (counters[2] != 0) return;  // an overflowed forward rendered nothing
+    const int tile = (int)b.active[blockIdx.x / chunks];
+    const int n = (int)b.tile_count[(size_t)tile * RTG_CNT_STRIDE];
+    if (n == 0) return;            // empty or masked-out tile
+    const int c0 = (int)(blockIdx.x % chunks) * K;
+    const int kc = min(K, C - c0);
+    int px, py;
+    bool inside;
+    pixel_of(vp, tile, px, py, inside);
+    const int pix = vp.W * py + px;
+    const size_t N = (size_t)vp.H * vp.W;
+    const int lane = threadIdx.x & 31;
+    const uint32_t last = inside ? img.n_contrib[pix] : 0u;
+    float G[K];
+#pragma unroll
+    for (int k = 0; k < K; k++) G[k] = (inside && k < kc) ? __ldg(dL_dout + (size_t)(c0 + k) * N + pix) : 0.f;
+    constexpr int SH = 5 - feat_log2<K>();
+    const int slot = lane >> SH;                                       // the channel this lane holds after the reduction
+    const bool writer = (lane & ((1 << SH) - 1)) == 0 && slot < kc;
+    auto stage = [](const int, const int) {};
+    auto visit = [&](const int j, const bool ok, const float wt) {
+        if (__ballot_sync(FULL, ok) == 0u) return;
+        float v[K];
+#pragma unroll
+        for (int k = 0; k < K; k++) v[k] = wt * G[k];  // wt = 0 on lanes that do not blend
+        const float s = warp_reduce_halving<K>(v, lane);
+        if (writer) atomicAdd(dL_dF + (size_t)sm.id[j] * C + c0 + slot, s);
+    };
+    replay_blends(vp, g, b, tile, last, (float)px, (float)py, sm, stage, visit);
+}
+
+// K channels per CTA: the smallest of 4, 8, 16 that holds C, 16 above that.
+template <int K>
+static void feat_launch(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img, const int32_t *counters,
+                        int C, const float *in, float *out, bool bwd, cudaStream_t s) {
+    const int chunks = (C + K - 1) / K;
+    const int grid = vp.tiles_x * vp.tiles_y * chunks;
+    if (bwd)
+        render_feat_bwd_kernel<K><<<grid, 256, 0, s>>>(vp, g, b, img, counters, C, chunks, in, out);
+    else
+        render_feat_fwd_kernel<K><<<grid, 256, 0, s>>>(vp, g, b, img, counters, C, chunks, in, out);
+}
+
+static void feat_dispatch(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                          const int32_t *counters, int C, const float *in, float *out, bool bwd, cudaStream_t s) {
+    if (C <= 4) feat_launch<4>(vp, g, b, img, counters, C, in, out, bwd, s);
+    else if (C <= 8) feat_launch<8>(vp, g, b, img, counters, C, in, out, bwd, s);
+    else feat_launch<16>(vp, g, b, img, counters, C, in, out, bwd, s);
+}
+
+void launch_render_features(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                            const int32_t *counters, int C, const float *features, float *out, cudaStream_t s) {
+    feat_dispatch(vp, g, b, img, counters, C, features, out, false, s);
+}
+
+void launch_render_features_bwd(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                                const int32_t *counters, int C, const float *dL_dout, float *dL_dfeatures, cudaStream_t s) {
+    feat_dispatch(vp, g, b, img, counters, C, dL_dout, dL_dfeatures, true, s);
+}
+
 }  // namespace rtg

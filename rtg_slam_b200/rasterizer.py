@@ -304,6 +304,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         color, depth, hit_color, hit_depth, hit_cw, hit_dw, T_map, radii = outs
         ctx.raster_settings = raster_settings
         ctx.native = saved
+        if _SAVED_SINK[0] is not None:
+            _SAVED_SINK[0].append(saved)
         ctx.provided = tuple(x is not None for x in inputs)
         ctx.camera_shapes = tuple(None if t is None else t.shape for t in (viewmatrix, projmatrix, campos))
         e = torch.empty(0, device=means3D.device)
@@ -425,6 +427,27 @@ class _RasterizeGaussians(torch.autograd.Function):
             return grads
         cam = (slice(0, 16), slice(16, 32), slice(32, 35))
         return grads + tuple(g_cam[c].reshape(s) if n else None for c, s, n in zip(cam, ctx.camera_shapes, ctx.needs_input_grad[9:]))
+
+
+# Optional list that receives the _Saved state of every forward (see `keep_saved`); None = not kept.
+_SAVED_SINK = [None]
+
+
+class keep_saved:
+    """Context manager: while active, every rasterizer forward appends its _Saved state (workspaces, counters, mode) to
+    the given list, so that a second pass can replay that forward (features.rasterize_features). Changes nothing else."""
+
+    def __init__(self, sink):
+        self.sink, self.prev = sink, None
+
+    def __enter__(self):
+        self.prev = _SAVED_SINK[0]
+        _SAVED_SINK[0] = self.sink
+        return self
+
+    def __exit__(self, *exc):
+        _SAVED_SINK[0] = self.prev
+        return False
 
 
 # Optional destination of the dense gradients (see `grad_buffers`); None = allocate per call.

@@ -427,6 +427,26 @@ int rtg_splat_features(const RtgSplatView *view, int32_t P, const void *geom_ws,
 int rtg_splat_features_backward(const RtgSplatView *view, int32_t P, const void *geom_ws, const void *img_ws,
                                 const void *bin_ws, int64_t R_cap, const int32_t *counters, int32_t C, const float *dL_dout,
                                 float *dL_dfeatures, void *stream);
+/* rtg_splat_features_backward_geometry: the other half of the feature map's gradient, through its blend weights. With
+ * h_i = sum_c dL_dout[c, p] features[i, c] and S_i = sum_{j > i} w_j h_j over the pixel's blended entries,
+ *   dL/dalpha_i = T_i h_i - S_i / (1 - alpha_i),
+ * taken through alpha to the same per-Gaussian gradients rtg_splat_backward gives (its colour backward with colours_precomp
+ * = features, bg = 0 and dL_ddepth = 0, summed over channel triples): dL_dmeans3D (P,3), dL_dopacity (P,1), and
+ * dL_dscales (P,3) + dL_drotations (P,4, 16-byte aligned) or dL_dcov3D (P,6), overwritten (culled rows 0, or unwritten
+ * with visible_rows_only != 0; radii is needed otherwise); with dL_dcamera (35 floats: view 16, proj 16, campos 3) and
+ * camera_scratch (rtg_splat_camera_scratch_bytes(P), 8-byte aligned) also the camera gradient, as
+ * rtg_splat_backward_camera. With every per-Gaussian output NULL and dL_dcamera given only the camera gradient is
+ * computed (rtg_splat_backward_pose's per-Gaussian half). means3D, scales / rotations or cov3D_precomp: the forward's
+ * inputs (no SH row and no opacity is read: opacities come from the forward's records). grad2d_scratch: P * 16 floats,
+ * zero on entry and on exit, as for every backward. dL/dfeatures comes from rtg_splat_features_backward. An overflowed
+ * forward gives zero gradients; P == 0 writes only dL_dcamera (zeros). Validates on the host before any CUDA work. */
+int rtg_splat_features_backward_geometry(const RtgSplatView *view, int32_t P, const float *means3D, const float *scales,
+                                         const float *rotations, const float *cov3D_precomp, const int32_t *radii,
+                                         const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap,
+                                         const int32_t *counters, int32_t C, const float *features, const float *dL_dout,
+                                         float *grad2d_scratch, float *dL_dmeans3D, float *dL_dopacity, float *dL_dscales,
+                                         float *dL_drotations, float *dL_dcov3D, int32_t visible_rows_only, float *dL_dcamera,
+                                         void *camera_scratch, void *stream);
 
 /* Replaces CudaRasterizer::Rasterizer::markVisible (rasterizer.h:21-26, rasterizer_impl.cu:145-157). */
 int rtg_splat_mark_visible(int32_t P, const float *means3D, const float *viewmatrix, const float *projmatrix,

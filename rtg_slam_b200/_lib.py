@@ -139,6 +139,10 @@ SIGNATURES = {
     # view, P, the three workspaces, R_cap, counters, C, input (features / dL_dout), output, stream
     "rtg_splat_features": (C.c_int, [C.POINTER(RtgSplatView), _I32] + [_VP] * 3 + [_I64, _VP, _I32] + [_VP] * 3),
     "rtg_splat_features_backward": (C.c_int, [C.POINTER(RtgSplatView), _I32] + [_VP] * 3 + [_I64, _VP, _I32] + [_VP] * 3),
+    # view, P, means3D, scales, rotations, cov3D_precomp, radii, the three workspaces, R_cap, counters, C, features, dL_dout,
+    # grad2d_scratch, five per-Gaussian gradients, visible_rows_only, dL_dcamera, camera_scratch, stream
+    "rtg_splat_features_backward_geometry": (C.c_int, [C.POINTER(RtgSplatView), _I32] + [_VP] * 5 + [_VP] * 3 + [_I64, _VP, _I32]
+                                             + [_VP] * 3 + [_VP] * 5 + [_I32, _VP, _VP, _VP]),
     "rtg_splat_pose_gn_step": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
                                + [C.POINTER(RtgPoseGN), _VP]),
     "rtg_splat_pose_gn_step_robust": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]

@@ -666,6 +666,76 @@ int rtg_splat_features_backward(const RtgSplatView *view, int32_t P, const void 
     return check_launch(who);
 }
 
+int rtg_splat_features_backward_geometry(const RtgSplatView *view, int32_t P, const float *means3D, const float *scales,
+                                         const float *rotations, const float *cov3D_precomp, const int32_t *radii,
+                                         const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap,
+                                         const int32_t *counters, int32_t C, const float *features, const float *dL_dout,
+                                         float *grad2d_scratch, float *dL_dmeans3D, float *dL_dopacity, float *dL_dscales,
+                                         float *dL_drotations, float *dL_dcov3D, int32_t visible_rows_only, float *dL_dcamera,
+                                         void *camera_scratch, void *stream) {
+    const char *who = "rtg_splat_features_backward_geometry";
+    auto bad = [&](const std::string &msg) { return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": " + msg); };
+    int rc = validate_view(view, who);
+    if (rc) return rc;
+    if (P < 0) return bad("P < 0");
+    if (R_cap < 0) return bad("R_cap < 0");
+    if (C < 1 || C > RTG_FEATURES_MAX)
+        return bad("C must be 1.." + std::to_string(RTG_FEATURES_MAX) + ", got " + std::to_string(C));
+    const bool per_gaussian = dL_dmeans3D || dL_dopacity || dL_dscales || dL_drotations || dL_dcov3D;
+    if (!per_gaussian && !dL_dcamera) return bad("no output: give the per-Gaussian gradients, dL_dcamera or both");
+    if (dL_dcamera && !camera_scratch) return bad("camera_scratch is NULL");
+    if (((uintptr_t)camera_scratch) & 7) return bad("camera_scratch must be 8-byte aligned");
+    if ((dL_dscales || dL_drotations) && (!scales || !rotations)) return bad("dL_dscales / dL_drotations without scales / rotations");
+    if (dL_dcov3D && !cov3D_precomp) return bad("dL_dcov3D without cov3D_precomp");
+    if ((((uintptr_t)features) | ((uintptr_t)dL_dout) | ((uintptr_t)dL_dmeans3D) | ((uintptr_t)dL_dopacity) |
+         ((uintptr_t)dL_dscales) | ((uintptr_t)dL_dcov3D) | ((uintptr_t)dL_dcamera)) & 3)
+        return bad("features / dL_dout / gradients must be 4-byte aligned");
+    if ((((uintptr_t)grad2d_scratch) | ((uintptr_t)rotations) | ((uintptr_t)dL_drotations)) & 15)
+        return bad("grad2d_scratch / rotations / dL_drotations must be 16-byte aligned");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    if (P == 0) {  // nothing visible: the camera gradient is zero, and there is no row to write
+        if (!dL_dcamera) return RTG_OK;
+        cudaError_t e = cudaMemsetAsync(dL_dcamera, 0, 35 * sizeof(float), s);
+        if (e != cudaSuccess) return fail(RTG_ERR_CUDA, std::string(who) + " memset: " + cudaGetErrorString(e));
+        return RTG_OK;
+    }
+    if (!geom_ws || !img_ws || !bin_ws || !counters) return bad("NULL workspace / counters");
+    if (!means3D || !features || !dL_dout || !grad2d_scratch) return bad("NULL means3D / features / dL_dout / grad2d_scratch");
+    if (((scales == nullptr || rotations == nullptr) && cov3D_precomp == nullptr) ||
+        ((scales != nullptr || rotations != nullptr) && cov3D_precomp != nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
+    if (per_gaussian) {
+        if (!dL_dmeans3D || !dL_dopacity) return bad("dL_dmeans3D / dL_dopacity is NULL");
+        if (scales && (!dL_dscales || !dL_drotations)) return bad("dL_dscales / dL_drotations is NULL");
+        if (cov3D_precomp && !dL_dcov3D) return bad("dL_dcov3D is NULL");
+        if (!visible_rows_only && !radii) return bad("radii is NULL (the culled rows are zero-filled from it)");
+    }
+    const rtg::ViewParams vp = make_view(view);
+    const int T = vp.tiles_x * vp.tiles_y;
+    rtg::GeomState g = rtg::geom_from(const_cast<void *>(geom_ws), (size_t)P);
+    rtg::ImgState img = rtg::img_from(const_cast<void *>(img_ws), (size_t)vp.H * vp.W);
+    rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
+    rtg::launch_render_features_grad(vp, g, b, img, counters, C, features, dL_dout, grad2d_scratch, s);
+    // the record holds moments only (no colour, no depth path): the per-Gaussian pass reads no SH row and writes no
+    // colour gradient
+    if (!per_gaussian) {
+        rtg::launch_preprocess_bwd_pose(vp, P, 0, means3D, scales, rotations, nullptr, cov3D_precomp, g, b.vis_count, grad2d_scratch,
+                                        dL_dcamera, camera_scratch, s);
+        return check_launch(who);
+    }
+    if (!visible_rows_only)
+        rtg::launch_bwd_zero(0, P, 0, false, cov3D_precomp == nullptr, radii, dL_dmeans3D, nullptr, nullptr, dL_dopacity, dL_dscales,
+                             dL_drotations, dL_dcov3D, nullptr, s);
+    if (dL_dcamera)
+        rtg::launch_preprocess_bwd_camera(vp, P, 0, means3D, scales, rotations, nullptr, cov3D_precomp, g, b.vis_count, grad2d_scratch,
+                                          dL_dmeans3D, nullptr, nullptr, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D, nullptr,
+                                          dL_dcamera, camera_scratch, s);
+    else
+        rtg::launch_preprocess_bwd(vp, P, 0, means3D, scales, rotations, nullptr, cov3D_precomp, g, b.vis_count, grad2d_scratch,
+                                   dL_dmeans3D, nullptr, nullptr, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D, nullptr, s);
+    return check_launch(who);
+}
+
 // The step of the Gauss-Newton entry points: `robust` selects the normal-equation rows (RTG_ROBUST_NONE: the plain ones),
 // `ab` (the device exposure, or nullptr) the eight-unknown step.
 static int pose_gn_step(const char *who, const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,

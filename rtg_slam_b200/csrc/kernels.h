@@ -66,6 +66,10 @@ void launch_render_features(const ViewParams &vp, const GeomState &g, const BinS
                             const int32_t *counters, int C, const float *features, float *out, cudaStream_t s);
 void launch_render_features_bwd(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
                                 const int32_t *counters, int C, const float *dL_dout, float *dL_dfeatures, cudaStream_t s);
+// the feature map's gradient through its blend weights: the six alpha moments added into the (zeroed) gradient record
+void launch_render_features_grad(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                                 const int32_t *counters, int C, const float *features, const float *dL_dout, float *rec,
+                                 cudaStream_t s);
 
 // mapstats.cu
 void launch_gs_error(int H, int W, int P, const float *color_err, const float *depth_err, const float *normal_err,

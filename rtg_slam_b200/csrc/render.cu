@@ -1614,6 +1614,129 @@ static void feat_dispatch(const ViewParams &vp, const GeomState &g, const BinSta
     else feat_launch<16>(vp, g, b, img, counters, C, in, out, bwd, s);
 }
 
+// Weight gradient: the feature map differentiated through its blend weights, with F and G = dL/dout held. For a pixel's
+// blended entries i (front to back), h_i = sum_c G[c] F[i, c] and S_i = sum_{j > i} w_j h_j,
+//   dL/dalpha_i = T_i h_i - S_i / (1 - alpha_i),
+// render_bwd_kernel's dL/dalpha with the pair's colour term D replaced by h_i and no background term. u = au dL/dalpha
+// feeds the six moments of the gradient record (REC_M0..REC_MYY), from where the per-Gaussian backward takes them to the
+// geometry and the camera. The replay runs front to back, so S_i = a - sum_{j <= i} w_j h_j with a = sum_j w_j h_j: a comes
+// from a first replay of the same tile in double, and the second replay subtracts the identical terms from it in the
+// identical order, in double, so what is left is the suffix sum to double rounding however far it cancels. (The
+// float map as a would carry an error of order 1e-7 |out| into every S_i, swamping the true S_i ~ T_i |h| of the entries
+// deep in a saturated pixel.) dL/dalpha is linear in h: each K-channel chunk adds its partial moments. Per (warp, entry)
+// with a blending lane the six sums go through warp_reduce_halving<8> and out as six REDs into the caller's zeroed record.
+// A pixel whose chunk of G is all zero adds nothing and is not replayed.
+template <int K>
+__global__ void __launch_bounds__(256) render_feat_grad_kernel(const ViewParams vp, const GeomState g, const BinState b,
+                                                               const ImgState img, const int *__restrict__ counters,
+                                                               const int C, const int chunks, const float *__restrict__ F,
+                                                               const float *__restrict__ dL_dout, float *__restrict__ rec) {
+    constexpr int FS = feat_stride<K>();
+    __shared__ ReplaySmem sm;
+    __shared__ __align__(16) float s_f[BATCH * FS];
+
+    if (counters[2] != 0) return;  // an overflowed forward rendered nothing
+    const int tile = (int)b.active[blockIdx.x / chunks];
+    const int n = (int)b.tile_count[(size_t)tile * RTG_CNT_STRIDE];
+    if (n == 0) return;            // empty or masked-out tile
+    const int c0 = (int)(blockIdx.x % chunks) * K;
+    const int kc = min(K, C - c0);
+    int px, py;
+    bool inside;
+    pixel_of(vp, tile, px, py, inside);
+    const int pix = vp.W * py + px;
+    const size_t N = (size_t)vp.H * vp.W;
+    const int lane = threadIdx.x & 31;
+    float G[K];
+    bool any = false;
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+        G[k] = (inside && k < kc) ? __ldg(dL_dout + (size_t)(c0 + k) * N + pix) : 0.f;
+        any |= G[k] != 0.f;
+    }
+    const uint32_t last = any ? img.n_contrib[pix] : 0u;
+    const float pxf = (float)px, pyf = (float)py;
+    auto stage = [&](const int slot, const int id) {
+        const float *row = F + (size_t)id * C + c0;
+        float v[K];
+#pragma unroll
+        for (int k = 0; k < K; k++) v[k] = k < kc ? __ldg(row + k) : 0.f;
+        float4 *dst = reinterpret_cast<float4 *>(s_f + slot * FS);
+#pragma unroll
+        for (int q = 0; q < K / 4; q++) dst[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+    };
+    auto h_of = [&](const int j) {
+        const float4 *row = reinterpret_cast<const float4 *>(s_f + j * FS);
+        float h = 0.f;
+#pragma unroll
+        for (int q = 0; q < K / 4; q++) {
+            const float4 f = row[q];
+            h = fmaf(G[4 * q], f.x, h);
+            h = fmaf(G[4 * q + 1], f.y, h);
+            h = fmaf(G[4 * q + 2], f.z, h);
+            h = fmaf(G[4 * q + 3], f.w, h);
+        }
+        return h;
+    };
+    double a = 0.0;
+    replay_blends(vp, g, b, tile, last, pxf, pyf, sm, stage, [&](const int j, const bool ok, const float wt) {
+        if (ok) a += (double)wt * (double)h_of(j);
+    });
+
+    constexpr int SH = 5 - feat_log2<8>();
+    const int slot = lane >> SH;                                   // the moment this lane holds after the reduction
+    const bool writer = (lane & ((1 << SH) - 1)) == 0 && slot < 6;
+    double rest = a;  // a - sum_{j <= i} w_j h_j = S_i, subtracted term by term in the order a was summed
+    float T = 1.f;
+    auto visit = [&](const int j, const bool ok, const float wt) {
+        if (__ballot_sync(FULL, ok) == 0u) return;
+        float v[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) v[k] = 0.f;
+        if (ok) {  // the replay's own decision and weight; its alpha and au are recomputed from the same inputs
+            const float4 s0 = sm.s0[j], s1 = sm.s1[j];
+            const float dx = s0.x - pxf, dy = s0.y - pyf;
+            float alpha, au;
+            pair_alpha(pair_power(s1.x, s1.y, s1.z, dx, dy), s1.w, s0.w, alpha, au);
+            const float h = h_of(j);
+            rest -= (double)wt * (double)h;
+            float inv_1ma;  // as in bwd_blend: 1 - alpha is in [0.01, 1], where the bare MUFU.RCP is exact to 1 ulp
+            asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv_1ma) : "f"(1.f - alpha));
+            const float dL_dalpha = T * h - (float)rest * inv_1ma;
+            T = T * (1.f - alpha);
+            const float u = au * dL_dalpha;
+            const float ux = u * dx, uy = u * dy;
+            v[0] = u;
+            v[1] = ux;
+            v[2] = uy;
+            v[3] = ux * dx;
+            v[4] = ux * dy;
+            v[5] = uy * dy;
+        }
+        const float s = warp_reduce_halving<8>(v, lane);
+        if (writer) atomicAdd(rec + (size_t)sm.id[j] * RTG_REC + REC_M0 + slot, s);
+    };
+    replay_blends(vp, g, b, tile, last, pxf, pyf, sm, stage, visit);
+}
+
+template <int K>
+static void feat_grad_launch(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                             const int32_t *counters, int C, const float *features, const float *dL_dout, float *rec,
+                             cudaStream_t s) {
+    const int chunks = (C + K - 1) / K;
+    render_feat_grad_kernel<K><<<vp.tiles_x * vp.tiles_y * chunks, 256, 0, s>>>(vp, g, b, img, counters, C, chunks, features,
+                                                                                dL_dout, rec);
+}
+
+void launch_render_features_grad(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                                 const int32_t *counters, int C, const float *features, const float *dL_dout, float *rec,
+                                 cudaStream_t s) {
+    // chunks of at most 8 channels: with 16, ptxas holds the kernel to 80 registers around the staging's division call
+    // (patch_mask) and spills
+    if (C <= 4) feat_grad_launch<4>(vp, g, b, img, counters, C, features, dL_dout, rec, s);
+    else feat_grad_launch<8>(vp, g, b, img, counters, C, features, dL_dout, rec, s);
+}
+
 void launch_render_features(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
                             const int32_t *counters, int C, const float *features, float *out, cudaStream_t s) {
     feat_dispatch(vp, g, b, img, counters, C, features, out, false, s);

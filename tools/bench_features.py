@@ -7,8 +7,10 @@ One frame: scene.surfel_room (seed 2024), all tiles, precomputed colours. render
 library's own per-kernel events (rtg_profile_enable) over N rasterizer forward + backward passes of the frame, which also
 give the device time of all the library's kernels of one such pass. Then, for C in 1, 3, 8, 16, 32, 64, 128 and N
 rounds, alternating within each round: the feature forward and the feature backward (its zero fill included) of that
-frame's saved state, each between two CUDA events, and the workaround, ceil(C / 3) GaussianRasterizer forward + backward
-passes with the features as `colors_precomp` three channels at a time, between two CUDA events. Medians are reported,
+frame's saved state, each between two CUDA events; the weight-gradient backward, dL/dF plus the geometry gradients through
+the blend weights (rtg_splat_features_backward + rtg_splat_features_backward_geometry, dense rows, no camera), between two
+CUDA events; and the workaround, ceil(C / 3) GaussianRasterizer forward + backward passes with the features as
+`colors_precomp` three channels at a time (which give both halves of that gradient), between two CUDA events. Medians are reported,
 after a few untimed rounds. Prints one JSON line with the card name, power limit and max SM clock read in the same run
 and the blended (pixel, Gaussian) pairs of the frame."""
 from __future__ import annotations
@@ -85,8 +87,8 @@ def main():
     res["blended_pairs"] = int(st["n_pixels"].sum().item())
 
     with torch.no_grad():
-        _, saved, _ = rasterizer._forward_native(rs, geo["means3D"], None, cols, geo["opacities"], geo["scales"],
-                                                 geo["rotations"], None, None)
+        outs, saved, _ = rasterizer._forward_native(rs, geo["means3D"], None, cols, geo["opacities"], geo["scales"],
+                                                    geo["rotations"], None, None)
     rasterizer._state(dev).read(saved.pending, block=True)
     assert not saved.pending.overflow
     view, keep = rasterizer._make_view(rs, dev, saved.antialiased)
@@ -115,6 +117,17 @@ def main():
         check(L.rtg_splat_features_backward(C.byref(view), P, *ws, c, C.c_void_p(G.data_ptr()), C.c_void_p(dF.data_ptr()),
                                             stream), "rtg_splat_features_backward")
 
+    record = rasterizer._state(dev).get_scratch(P)
+    grads = [torch.empty((P, k), device=dev) for k in (3, 1, 3, 4)]
+    vp = lambda t: C.c_void_p(t.data_ptr())
+
+    def weight_bwd(c):
+        feat_bwd(c)
+        F, G = data[c][0], data[c][1]
+        check(L.rtg_splat_features_backward_geometry(
+            C.byref(view), P, vp(geo["means3D"]), vp(geo["scales"]), vp(geo["rotations"]), None, vp(outs[7]), *ws, c, vp(F),
+            vp(G), vp(record), *[vp(t) for t in grads], None, 0, None, None, stream), "rtg_splat_features_backward_geometry")
+
     def workaround(c):
         for Fk, Gk in data[c][4]:
             rasterizer_pass(Fk, Gk)
@@ -127,10 +140,10 @@ def main():
         t.synchronize()
         return s.elapsed_time(t)
 
-    times = {c: {"fwd": [], "bwd": [], "workaround": []} for c in CHANNELS}
+    times = {c: {"fwd": [], "bwd": [], "weight_bwd": [], "workaround": []} for c in CHANNELS}
     for i in range(a.warmup + a.iters):
         for c in CHANNELS:
-            for key, fn in (("fwd", feat_fwd), ("bwd", feat_bwd), ("workaround", workaround)):
+            for key, fn in (("fwd", feat_fwd), ("bwd", feat_bwd), ("weight_bwd", weight_bwd), ("workaround", workaround)):
                 ms = timed(fn, c)
                 if i >= a.warmup:
                     times[c][key].append(ms)
@@ -142,7 +155,10 @@ def main():
                         "features_total_ms": round(total, 4), "workaround_passes": -(-c // 3),
                         "workaround_ms": round(med["workaround"], 4), "speedup": round(med["workaround"] / total, 2),
                         "fwd_ratio_to_render_fwd": round(med["fwd"] / per["render_fwd"], 3),
-                        "bwd_ratio_to_render_bwd": round(med["bwd"] / per["render_bwd"], 3)}
+                        "bwd_ratio_to_render_bwd": round(med["bwd"] / per["render_bwd"], 3),
+                        "weight_bwd_ms": round(med["weight_bwd"], 4),
+                        "weight_total_ms": round(med["fwd"] + med["weight_bwd"], 4),
+                        "weight_speedup": round(med["workaround"] / (med["fwd"] + med["weight_bwd"]), 2)}
     res["channels"] = rows
     torch.cuda.synchronize()
     print(json.dumps(res))

@@ -590,6 +590,28 @@ int rtg_icp_predict_pose(const RtgIcpLevel *levels, int32_t n_levels, float dist
                          const float *p2p_normal_t0, int32_t p2p_H, int32_t p2p_W, float *out, float *out_host, void *ws,
                          void *stream);
 
+/* Intensity pyramid of the photometric ICP term, all levels in one launch. `color`: device float32, (H,W,3) if
+ * channels_last else (3,H,W). Level l, intensity_out[l] (device, (H/pools[l], W/pools[l]) floats), holds per pixel the mean
+ * of Y = 0.299 R + 0.587 G + 0.114 B over the pools[l] x pools[l] block whose maximum rtg_icp_build_pyramid takes for the
+ * depth: the same pixel grid and level intrinsics. 1 <= n_levels <= 4. Validated on the host before any CUDA work. */
+int rtg_icp_build_intensity_pyramid(const float *color, int32_t H, int32_t W, int32_t channels_last, int32_t n_levels,
+                                    const int32_t *pools, float *const *intensity_out, void *stream);
+
+/* rtg_icp_predict_pose with a photometric term (RGB-D odometry), one cooperative launch as well. For every pixel whose
+ * geometric row is valid, the row r = I1(u,v) - I0[q] is added: I1 is the bilinear interpolation of the previous frame's
+ * level intensity intensity1[l] at the projection (u,v) of the geometric row, I0 = intensity0[l] the current frame's;
+ * J = (v' x a, a) with a = dr/dv' through the exact derivative of the interpolant. H = sum_geo J^T J +
+ * photometric_weight * sum_photo J^T J, g likewise; damping, solve and update as in rtg_icp_predict_pose. intensity0[l] /
+ * intensity1[l]: device, (levels[l].H, levels[l].W) floats (rtg_icp_build_intensity_pyramid). photometric_weight: m^2 per
+ * squared intensity unit, finite and >= 0; with 0 the 18 leading floats are rtg_icp_predict_pose's, bit for bit.
+ * out / out_host: 20 floats = the 18 of rtg_icp_predict_pose, then the photometric ratio (count / (H*W) of the level) and
+ * RMS residual (0 without rows) of the last iteration. Arguments are validated on the host before any CUDA work. */
+int rtg_icp_predict_pose_rgbd(const RtgIcpLevel *levels, const float *const *intensity0, const float *const *intensity1,
+                              int32_t n_levels, float distance_threshold, float normal_cos_threshold, float damping,
+                              float photometric_weight, const float *pose_init, const float *p2p_vertex_t0,
+                              const float *p2p_vertex_t1, const float *p2p_normal_t0, int32_t p2p_H, int32_t p2p_W, float *out,
+                              float *out_host, void *ws, void *stream);
+
 /* ---- image-space glue between the rasterizer forward and backward (SURVEY.md section 8(f) #1) -------------
  * Fused masked L1 colour + depth loss of Mapping.loss_update (SLAM/multiprocess/mapper.py:402-431,444-451, with
  * l1_loss of utils/loss_utils.py:27-31) and its gradients w.r.t. the rendered colour and depth:

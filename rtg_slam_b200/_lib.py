@@ -160,6 +160,11 @@ SIGNATURES = {
     "rtg_icp_solve_level": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _F, _F, _F, _F, _F, _F, _F, _I32, _VP, _VP, _VP, _VP]),
     "rtg_icp_build_pyramid": (C.c_int, [_VP, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "rtg_icp_predict_pose": (C.c_int, [_VP, _I32, _F, _F, _F, _VP, _VP, _VP, _VP, _I32, _I32, _VP, _VP, _VP, _VP]),
+    # color, H, W, channels_last, n_levels, pools, intensity_out, stream
+    "rtg_icp_build_intensity_pyramid": (C.c_int, [_VP, _I32, _I32, _I32, _I32, _VP, _VP, _VP]),
+    # levels, intensity0, intensity1, then rtg_icp_predict_pose's arguments with photometric_weight after damping
+    "rtg_icp_predict_pose_rgbd": (C.c_int, [_VP, _VP, _VP, _I32, _F, _F, _F, _F, _VP, _VP, _VP, _VP, _I32, _I32, _VP, _VP, _VP,
+                                            _VP]),
     "rtg_icp_point2plane_loss": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _VP, _VP, _VP, _VP]),
     "rtg_icp_fill_model_depth": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _F, _F, _VP]),
     "rtg_loss_workspace_bytes": (C.c_size_t, []),

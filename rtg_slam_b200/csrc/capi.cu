@@ -975,6 +975,57 @@ int rtg_icp_predict_pose(const RtgIcpLevel *levels, int32_t n_levels, float dist
     return check_launch("rtg_icp_predict_pose");
 }
 
+int rtg_icp_build_intensity_pyramid(const float *color, int32_t H, int32_t W, int32_t channels_last, int32_t n_levels,
+                                    const int32_t *pools, float *const *intensity_out, void *stream) {
+    if (!color || !pools || !intensity_out || H <= 0 || W <= 0 || n_levels < 1 || n_levels > RTG_ICP_MAX_LEVELS)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_icp_build_intensity_pyramid: bad arguments");
+    rtg::IcpIntensity p;
+    p.color = color; p.H = H; p.W = W; p.channels_last = channels_last ? 1 : 0; p.n_levels = n_levels;
+    int64_t total = 0;
+    for (int l = 0; l < n_levels; l++) {
+        if (pools[l] < 1 || H / pools[l] < 1 || W / pools[l] < 1 || !intensity_out[l])
+            return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_icp_build_intensity_pyramid: bad level");
+        p.pool[l] = pools[l]; p.out[l] = intensity_out[l]; p.start[l] = (int)total;
+        total += (int64_t)(H / pools[l]) * (W / pools[l]);
+    }
+    if (total > INT32_MAX) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_icp_build_intensity_pyramid: frame too large");
+    for (int l = n_levels; l < RTG_ICP_MAX_LEVELS; l++) { p.pool[l] = 1; p.out[l] = nullptr; p.start[l] = (int)total; }
+    p.total = (int)total;
+    rtg::launch_icp_intensity_pyramid(p, reinterpret_cast<cudaStream_t>(stream));
+    return check_launch("rtg_icp_build_intensity_pyramid");
+}
+
+int rtg_icp_predict_pose_rgbd(const RtgIcpLevel *levels, const float *const *intensity0, const float *const *intensity1,
+                              int32_t n_levels, float distance_threshold, float normal_cos_threshold, float damping,
+                              float photometric_weight, const float *pose_init, const float *p2p_vertex_t0,
+                              const float *p2p_vertex_t1, const float *p2p_normal_t0, int32_t p2p_H, int32_t p2p_W, float *out,
+                              float *out_host, void *ws, void *stream) {
+    if (!levels || !intensity0 || !intensity1 || n_levels < 1 || n_levels > RTG_ICP_MAX_LEVELS || !p2p_vertex_t0 ||
+        !p2p_vertex_t1 || !p2p_normal_t0 || p2p_H <= 0 || p2p_W <= 0 || !out || !ws)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_icp_predict_pose_rgbd: bad arguments");
+    if (!(photometric_weight >= 0.f) || !std::isfinite(photometric_weight))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_icp_predict_pose_rgbd: photometric_weight must be finite and >= 0");
+    rtg::IcpPredict p;
+    rtg::IcpPhoto ph{};
+    p.n_levels = n_levels;
+    for (int l = 0; l < n_levels; l++) {
+        const RtgIcpLevel &L = levels[l];
+        if (!L.vertex0 || !L.normal0 || !L.vertex1 || !L.normal1 || L.H <= 0 || L.W <= 0 || L.iters < 0 || !intensity0[l] ||
+            !intensity1[l])
+            return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_icp_predict_pose_rgbd: bad level");
+        p.lv[l] = rtg::IcpLevel{L.vertex0, L.normal0, L.vertex1, L.normal1, L.H, L.W, L.fx, L.fy, L.cx, L.cy, L.iters};
+        ph.I0[l] = intensity0[l]; ph.I1[l] = intensity1[l];
+    }
+    ph.w = photometric_weight;
+    p.dist_thr = distance_threshold; p.cos_thr = normal_cos_threshold; p.damping = damping;
+    p.pose_in = pose_init;
+    p.p2p_v_t0 = p2p_vertex_t0; p.p2p_v_t1 = p2p_vertex_t1; p.p2p_n_t0 = p2p_normal_t0; p.p2p_HW = p2p_H * p2p_W;
+    p.out = out; p.out_host = out_host;
+    cudaError_t e = rtg::launch_icp_predict_rgbd(p, ph, ws, reinterpret_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return fail(RTG_ERR_CUDA, std::string("rtg_icp_predict_pose_rgbd: ") + cudaGetErrorString(e));
+    return check_launch("rtg_icp_predict_pose_rgbd");
+}
+
 int rtg_icp_point2plane_loss(const float *vertex_t0, const float *vertex_t1, const float *normal_t0, int32_t H, int32_t W,
                              const float *pose, float *loss, void *ws, void *stream) {
     if (!vertex_t0 || !vertex_t1 || !normal_t0 || !pose || !loss || !ws || H <= 0 || W <= 0)

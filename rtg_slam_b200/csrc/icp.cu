@@ -6,6 +6,7 @@
 // iteration computes the per-pixel residual and Jacobian row, reduces the 27 unique normal-equation
 // terms (+ valid count) by a transposing warp butterfly and per-block double partials, and the last
 // block to finish solves the damped 6x6 system, applies exp_se3 and updates the pose in place.
+// icp_predict_kernel<true> adds a photometric row (RGB-D odometry) to the same normal equations.
 #include "common.cuh"
 #include "kernels.h"
 #include "prof.h"
@@ -15,7 +16,7 @@ namespace rtg {
 
 #define ICP_THREADS 256
 #define ICP_MAX_BLOCKS (RTG_NUM_SMS * 4)
-#define ICP_TERMS 32        // 21 (JtJ upper) + 6 (Jtr) + 1 (valid) padded to 32
+#define ICP_TERMS 32        // 21 (JtJ upper) + 6 (Jtr) + 1 (valid) [+ 2 (photometric count, sum r^2)] padded to 32
 
 #define ICP_MAX_LEVELS RTG_ICP_MAX_LEVELS
 struct IcpWs {
@@ -377,9 +378,15 @@ __device__ __forceinline__ void grid_barrier(unsigned int *counter, unsigned int
 }
 
 // Per-pixel residual and Jacobian row of one iteration, accumulated into the 28 normal-equation terms (same arithmetic
-// as icp_iter_kernel above; `pose` in shared memory).
+// as icp_iter_kernel above; `pose` in shared memory). With RGBD, every pixel with a valid geometric row also adds the
+// photometric row: r = I1(u, v) - I0[p], bilinear in the previous frame's level intensity at the projection the
+// geometric row already computed, with J = (v' x a, a), a = dr/dv' through the exact derivative of the interpolant. Its
+// terms enter the same 27 slots scaled by photo_w (after the geometric ones, so photo_w = 0 leaves every slot's bits
+// unchanged); slots 28 and 29 take its count and its sum of r^2.
+template <bool RGBD>
 __device__ __forceinline__ void icp_accumulate(const IcpLevel &L, const float *pose, const float dist_thr, const float cos_thr,
-                                               float acc[ICP_TERMS]) {
+                                               float acc[ICP_TERMS], const float *__restrict__ inten0 = nullptr,
+                                               const float *__restrict__ inten1 = nullptr, const float photo_w = 0.f) {
     float Rm[9], tv[3];
 #pragma unroll
     for (int i = 0; i < 3; i++) {
@@ -433,6 +440,36 @@ __device__ __forceinline__ void icp_accumulate(const IcpLevel &L, const float *p
 #pragma unroll
             for (int a = 0; a < 6; a++) acc[21 + a] += J[a] * res;
             acc[27] += 1.f;
+            if constexpr (RGBD) {
+                // 0 < u < W-1 and 0 < v < H-1 (inview): the four taps exist
+                const float fu = floorf(u), fv = floorf(v);
+                const float al = u - fu, be = v - fv;
+                const size_t t = (size_t)(int)fv * W + (int)fu;
+                const float i00 = inten1[t], i10 = inten1[t + 1], i01 = inten1[t + W], i11 = inten1[t + W + 1];
+                const float I = (1.f - be) * ((1.f - al) * i00 + al * i10) + be * ((1.f - al) * i01 + al * i11);
+                const float r = I - inten0[p];
+                const float gu = (1.f - be) * (i10 - i00) + be * (i11 - i01);
+                const float gv = (1.f - al) * (i01 - i00) + al * (i11 - i10);
+                const float iz = 1.f / z;
+                const float a0 = gu * fx * iz, a1 = gv * fy * iz, a2 = -(a0 * x + a1 * y) * iz;
+                float Jp[6];
+                Jp[0] = y * a2 - z * a1;
+                Jp[1] = z * a0 - x * a2;
+                Jp[2] = x * a1 - y * a0;
+                Jp[3] = a0; Jp[4] = a1; Jp[5] = a2;
+                float Jw[6];
+#pragma unroll
+                for (int a = 0; a < 6; a++) Jw[a] = photo_w * Jp[a];
+                int kp = 0;
+#pragma unroll
+                for (int a = 0; a < 6; a++)
+#pragma unroll
+                    for (int c = a; c < 6; c++) acc[kp++] += Jw[a] * Jp[c];
+#pragma unroll
+                for (int a = 0; a < 6; a++) acc[21 + a] += Jw[a] * r;
+                acc[28] += 1.f;
+                acc[29] += r * r;
+            }
         }
     }
 }
@@ -469,16 +506,23 @@ __device__ __forceinline__ void icp_grid_total(const double *partial, double (*s
 // IcpTracker.predict_pose in one cooperative launch (SLAM/icp.py:417-452): for every pyramid level, `iters` Gauss-Newton
 // iterations (one grid barrier each: every block reduces the per-block partial sums itself and solves the 6x6 system
 // redundantly, so the updated pose needs no broadcast), then the point-to-plane loss of the final pose; pose (16),
-// loss and valid ratio go to `out` on the device and, if given, straight into mapped host memory.
-__global__ void __launch_bounds__(ICP_P_THREADS) icp_predict_kernel(const IcpPredict prm, IcpWs *ws) {
+// loss and valid ratio go to `out` on the device and, if given, straight into mapped host memory. RGBD adds the
+// photometric row (icp_accumulate) and two more result floats: the photometric ratio and RMS residual of the last
+// iteration.
+template <bool RGBD>
+__global__ void __launch_bounds__(ICP_P_THREADS) icp_predict_kernel(const IcpPredict prm, IcpWs *ws, const IcpPhoto ph) {
     __shared__ float s_red[ICP_P_THREADS / 32][ICP_TERMS];
     __shared__ double s_part[ICP_P_THREADS / 32][ICP_TERMS];
     __shared__ double s_tot[ICP_TERMS];
     __shared__ float s_pose[16];
     __shared__ float s_valid;
+    __shared__ float s_photo[2];
     unsigned int generation = 0;
     if (threadIdx.x < 16) s_pose[threadIdx.x] = prm.pose_in ? prm.pose_in[threadIdx.x] : ((threadIdx.x % 5 == 0) ? 1.f : 0.f);
     if (threadIdx.x == 0) s_valid = 0.f;
+    if constexpr (RGBD) {
+        if (threadIdx.x < 2) s_photo[threadIdx.x] = 0.f;
+    }
     __syncthreads();
     int it_global = 0;
     for (int l = 0; l < prm.n_levels; l++) {
@@ -487,7 +531,15 @@ __global__ void __launch_bounds__(ICP_P_THREADS) icp_predict_kernel(const IcpPre
             float acc[ICP_TERMS];
 #pragma unroll
             for (int k = 0; k < ICP_TERMS; k++) acc[k] = 0.f;
-            icp_accumulate(L, s_pose, prm.dist_thr, prm.cos_thr, acc);
+            if constexpr (RGBD) {
+                // constant indices only, so the intensity pointers stay in the constant bank
+                const float *i0 = ph.I0[0], *i1 = ph.I1[0];
+#pragma unroll
+                for (int j = 1; j < ICP_MAX_LEVELS; j++)
+                    if (j == l) { i0 = ph.I0[j]; i1 = ph.I1[j]; }
+                icp_accumulate<true>(L, s_pose, prm.dist_thr, prm.cos_thr, acc, i0, i1, ph.w);
+            } else
+                icp_accumulate<false>(L, s_pose, prm.dist_thr, prm.cos_thr, acc);
             double *partial = (it_global & 1) ? ws->partial2 : ws->partial;
             icp_block_partial(acc, s_red, partial + (size_t)blockIdx.x * ICP_TERMS);
             grid_barrier(&ws->barrier, generation);
@@ -505,6 +557,10 @@ __global__ void __launch_bounds__(ICP_P_THREADS) icp_predict_kernel(const IcpPre
                 for (int a = 0; a < 6; a++) { A[a][a] += trace * (double)prm.damping; bvec[a] = -s_tot[21 + a]; }
                 if (solve6(A, bvec, xi)) se3_update(xi, s_pose);
                 s_valid = (float)(s_tot[27] / (double)L.H / (double)L.W);
+                if constexpr (RGBD) {
+                    s_photo[0] = (float)(s_tot[28] / (double)L.H / (double)L.W);
+                    s_photo[1] = s_tot[28] > 0.0 ? (float)sqrt(s_tot[29] / s_tot[28]) : 0.f;
+                }
             }
             __syncthreads();
         }
@@ -556,6 +612,12 @@ __global__ void __launch_bounds__(ICP_P_THREADS) icp_predict_kernel(const IcpPre
             } else if (threadIdx.x == 17) {
                 prm.out[17] = s_valid;
                 if (prm.out_host) prm.out_host[17] = s_valid;
+            }
+            if constexpr (RGBD) {
+                if (threadIdx.x == 18 || threadIdx.x == 19) {
+                    prm.out[threadIdx.x] = s_photo[threadIdx.x - 18];
+                    if (prm.out_host) prm.out_host[threadIdx.x] = s_photo[threadIdx.x - 18];
+                }
             }
         }
     }
@@ -626,6 +688,35 @@ __global__ void __launch_bounds__(256) icp_pyramid_kernel(const IcpPyramid prm, 
     }
 }
 
+// Intensity pyramid of the photometric term, all levels in one launch: one thread per level pixel, the mean of
+// Y = 0.299 R + 0.587 G + 0.114 B over the pool x pool block whose maximum icp_pyramid_kernel takes for the depth.
+__global__ void __launch_bounds__(256) icp_intensity_pyramid_kernel(const IcpIntensity prm) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= prm.total) return;
+    // constant indices only, so the parameter arrays stay in the constant bank
+    int start = 0, pool = prm.pool[0];
+    float *out = prm.out[0];
+#pragma unroll
+    for (int j = 1; j < RTG_ICP_MAX_LEVELS; j++)
+        if (j < prm.n_levels && idx >= prm.start[j]) { start = prm.start[j]; pool = prm.pool[j]; out = prm.out[j]; }
+    const int Ws = prm.W / pool, H = prm.H, W = prm.W;
+    const int k = idx - start, ys = k / Ws, xs = k % Ws;
+    const size_t plane = (size_t)H * W;
+    float s = 0.f;
+    for (int a = 0; a < pool; a++)
+        for (int c = 0; c < pool; c++) {
+            const size_t q = (size_t)(ys * pool + a) * W + xs * pool + c;
+            float R, G, B;
+            if (prm.channels_last) {
+                R = prm.color[3 * q]; G = prm.color[3 * q + 1]; B = prm.color[3 * q + 2];
+            } else {
+                R = prm.color[q]; G = prm.color[plane + q]; B = prm.color[2 * plane + q];
+            }
+            s += 0.299f * R + 0.587f * G + 0.114f * B;
+        }
+    out[k] = s / (float)(pool * pool);
+}
+
 __global__ void icp_persistent_init_kernel(IcpWs *ws) {
     ws->barrier = 0;
     if (threadIdx.x < ICP_MAX_LEVELS) {
@@ -643,14 +734,28 @@ static int sm_count() {
     return n[dev] > 0 ? n[dev] : 1;
 }
 
-cudaError_t launch_icp_predict(const IcpPredict &prm, void *ws_, cudaStream_t s) {
+template <bool RGBD>
+static cudaError_t launch_icp_predict_t(const IcpPredict &prm, const IcpPhoto &ph, void *ws_, cudaStream_t s) {
     IcpWs *ws = reinterpret_cast<IcpWs *>(ws_);
     ProfScope ps(K_ICP_ITER, s);
     icp_persistent_init_kernel<<<1, 32, 0, s>>>(ws);
     int grid = sm_count();
     if (grid > ICP_MAX_BLOCKS) grid = ICP_MAX_BLOCKS;
-    void *args[] = {(void *)&prm, (void *)&ws};
-    return cudaLaunchCooperativeKernel((const void *)icp_predict_kernel, dim3(grid), dim3(ICP_P_THREADS), args, 0, s);
+    void *args[] = {(void *)&prm, (void *)&ws, (void *)&ph};
+    return cudaLaunchCooperativeKernel((const void *)icp_predict_kernel<RGBD>, dim3(grid), dim3(ICP_P_THREADS), args, 0, s);
+}
+
+cudaError_t launch_icp_predict(const IcpPredict &prm, void *ws, cudaStream_t s) {
+    const IcpPhoto none{};
+    return launch_icp_predict_t<false>(prm, none, ws, s);
+}
+
+cudaError_t launch_icp_predict_rgbd(const IcpPredict &prm, const IcpPhoto &ph, void *ws, cudaStream_t s) {
+    return launch_icp_predict_t<true>(prm, ph, ws, s);
+}
+
+void launch_icp_intensity_pyramid(const IcpIntensity &prm, cudaStream_t s) {
+    icp_intensity_pyramid_kernel<<<(prm.total + 255) / 256, 256, 0, s>>>(prm);
 }
 
 cudaError_t launch_icp_pyramid(const IcpPyramid &prm, void *ws_, cudaStream_t s) {

@@ -102,6 +102,20 @@ struct IcpPredict {
     int p2p_HW;
     float *out, *out_host;
 };
+// photometric term of icp_predict_kernel<true>: per-level intensities of the current ("0") and previous ("1") frame,
+// each (H, W) of its level, and the weight of the photometric normal equations (out then holds 20 floats)
+struct IcpPhoto {
+    const float *I0[RTG_ICP_MAX_LEVELS], *I1[RTG_ICP_MAX_LEVELS];
+    float w;
+};
+struct IcpIntensity {
+    const float *color;  // (H, W, 3) if channels_last, else (3, H, W)
+    int H, W, channels_last, n_levels;
+    int pool[RTG_ICP_MAX_LEVELS];
+    int start[RTG_ICP_MAX_LEVELS];  // first thread of each level
+    int total;                      // level pixels of all levels
+    float *out[RTG_ICP_MAX_LEVELS];
+};
 struct IcpPyramid {
     const float *depth;
     int H, W, n_levels;
@@ -110,7 +124,9 @@ struct IcpPyramid {
     float *vertex[RTG_ICP_MAX_LEVELS], *normal[RTG_ICP_MAX_LEVELS];
 };
 cudaError_t launch_icp_predict(const IcpPredict &prm, void *ws, cudaStream_t s);
+cudaError_t launch_icp_predict_rgbd(const IcpPredict &prm, const IcpPhoto &ph, void *ws, cudaStream_t s);
 cudaError_t launch_icp_pyramid(const IcpPyramid &prm, void *ws, cudaStream_t s);
+void launch_icp_intensity_pyramid(const IcpIntensity &prm, cudaStream_t s);
 
 // mapsurgery.cu
 #ifndef RTG_SOA_MAX_ARRAYS

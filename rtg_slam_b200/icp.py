@@ -5,7 +5,8 @@ the reference (SLAM/icp.py:16-48,357-452); the arithmetic runs in librtg_splat_b
 is ONE cooperative kernel (all levels x all Gauss-Newton iterations: residuals + Jacobians + 27-term reduction +
 damped 6x6 solve + exp_se3 + pose update, one grid barrier per iteration, then the point-to-plane loss) that writes
 its 72-byte result straight into pinned host memory, and a pyramid is one launch, against ~600 eager ops and >= 45
-host synchronisations in the reference. `ICP.icp` (one level) keeps the kernel-per-iteration entry point."""
+host synchronisations in the reference. `ICP.icp` (one level) keeps the kernel-per-iteration entry point.
+`RgbdIcpTracker` (no counterpart in the reference) adds a photometric term to the same one-launch loop."""
 from __future__ import annotations
 
 import ctypes as C
@@ -222,5 +223,136 @@ class IcpTracker:
         self.last_p2ploss, self.last_valid_ratio = float(host[16]), float(host[17])
         if self.verbose:
             print(self.last_p2ploss, self.last_valid_ratio)
+        tracking_success = not (self.last_p2ploss > self.icp_fail_threshold)
+        return pose_t1_t0, tracking_success
+
+
+# ---------------------------------------------------------------------------------------------------- RGB-D tracking
+_RES_RGBD = {}
+
+
+def _result_buffers_rgbd(device):
+    """(device 20 floats, mapped pinned 20 floats, event) of RgbdIcpTracker.predict_pose, one set per device."""
+    idx = device.index if device.index is not None else torch.cuda.current_device()
+    if idx not in _RES_RGBD:
+        _RES_RGBD[idx] = (torch.zeros(20, dtype=torch.float32, device=torch.device("cuda", idx)),
+                          torch.zeros(20, dtype=torch.float32).pin_memory(), torch.cuda.Event())
+    return _RES_RGBD[idx]
+
+
+def _color_layout(color, H, W):
+    """True for (H, W, 3), False for (3, H, W); TypeError / ValueError before any CUDA work otherwise."""
+    if not isinstance(color, torch.Tensor) or not color.is_cuda or color.dtype != torch.float32:
+        raise TypeError("color must be a CUDA float32 tensor, (H, W, 3) or (3, H, W)")
+    if color.dim() == 3 and tuple(color.shape) == (H, W, 3):
+        return True
+    if color.dim() == 3 and tuple(color.shape) == (3, H, W):
+        return False
+    raise ValueError(f"color must be (H, W, 3) or (3, H, W) with (H, W) = ({H}, {W}) of the depth; got {tuple(color.shape)}")
+
+
+def build_intensity_pyramid(color, n_levels):
+    """Intensity pyramid of the photometric ICP term, index 0 the coarsest level like build_pyramids: level i has
+    pool p = 2**(n_levels-1-i) and (H//p, W//p) pixels, each the mean of Y = 0.299 R + 0.587 G + 0.114 B over the p x p
+    block whose depth maximum build_pyramids takes. `color`: CUDA float32, (H, W, 3) or (3, H, W). One launch."""
+    if not isinstance(color, torch.Tensor) or color.dim() != 3:
+        raise TypeError("color must be a CUDA float32 tensor, (H, W, 3) or (3, H, W)")
+    if not 1 <= n_levels <= 4:
+        raise ValueError("1 to 4 pyramid levels")
+    H, W = (color.shape[0], color.shape[1]) if color.shape[-1] == 3 else (color.shape[1], color.shape[2])
+    channels_last = _color_layout(color, H, W)
+    c = color.contiguous()
+    pools = [1 << (n_levels - 1 - i) for i in range(n_levels)]
+    out = [torch.empty((H // p, W // p), dtype=torch.float32, device=c.device) for p in pools]
+    I32, VP = C.c_int32 * n_levels, C.c_void_p * n_levels
+    check(_lib.lib().rtg_icp_build_intensity_pyramid(_p(c), H, W, 1 if channels_last else 0, n_levels, I32(*pools),
+                                                     VP(*[o.data_ptr() for o in out]), _stream(c.device)),
+          "rtg_icp_build_intensity_pyramid")
+    return out
+
+
+class RgbdIcpTracker(IcpTracker):
+    """IcpTracker with a photometric term in the same Gauss-Newton loop (RGB-D odometry as in ElasticFusion / DVO).
+
+    Per pixel with a valid point-to-plane row, r = I_prev(u, v) - I_curr[q] at the projection the geometric row
+    computes, bilinear in the previous frame's level intensity; H = sum_geo J^T J + photometric_weight * sum_photo J^T J
+    (and g alike). `photometric_weight` is in m^2 per squared intensity unit; the default 0.01 = (2 mm / 0.02)^2 is the
+    ratio of sensor depth noise to intensity noise. Frames without colour, or a weight of 0, track exactly as IcpTracker.
+    In frame-to-model mode the model depth is IcpTracker's and the model intensity is the previous frame's measured one
+    (the render is made at that frame's tracked pose, so it shares its pixel grid)."""
+
+    def __init__(self, args, photometric_weight=0.01):
+        w = float(photometric_weight)
+        if not (w >= 0.0 and np.isfinite(w)):
+            raise ValueError("photometric_weight must be finite and >= 0")
+        super().__init__(args)
+        self.photometric_weight = w
+        self.intensity_pyramid_t0 = None
+        self.intensity_pyramid_t1 = None
+        self.last_photometric_ratio = None
+        self.last_photometric_rmse = None
+
+    def update_curr_status(self, depth_t1, K, color_t1=None):
+        if color_t1 is not None:  # checked before any CUDA work
+            if not isinstance(depth_t1, torch.Tensor):
+                raise TypeError("depth_t1 must be a CUDA float32 tensor")
+            _color_layout(color_t1, depth_t1.shape[0], depth_t1.shape[1])
+        super().update_curr_status(depth_t1, K)
+        self.intensity_pyramid_t1 = None if color_t1 is None else build_intensity_pyramid(color_t1, len(self.icp_downscales))
+
+    def move_last_status(self):
+        super().move_last_status()
+        self.intensity_pyramid_t0 = self.intensity_pyramid_t1
+
+    def predict_pose(self, frame):
+        if (self.vertex_pyramid_t0 is None or self.intensity_pyramid_t0 is None or self.intensity_pyramid_t1 is None
+                or not self.photometric_weight > 0.0):
+            self.last_photometric_ratio, self.last_photometric_rmse = 0.0, 0.0
+            return super().predict_pose(frame)
+        K = frame["K"]
+        frame_id = frame["frame_id"]
+        L = _lib.lib()
+        levels = len(self.icp_downscales)
+        if self.icp_use_model_depth and frame_id >= self.icp_warmup_frames:
+            self.vertex_pyramid_t0, self.normal_pyramid_t0 = build_pyramids(self.last_model_depth, self._Kf, levels)
+        device = self.vertex_pyramid_t1[0].device
+        Kf = _intrinsics(K) if K is not self.K else self._Kf
+        lv = (_lib.RtgIcpLevel * levels)()
+        VP = C.c_void_p * levels
+        i0 = VP(*[self.intensity_pyramid_t1[level].data_ptr() for level in range(levels)])
+        i1 = VP(*[self.intensity_pyramid_t0[level].data_ptr() for level in range(levels)])
+        keep = []
+        for level in range(levels):
+            s = np.float32(self.icp_downscales[level])
+            # "0" inside the solve is the CURRENT frame, as in IcpTracker.predict_pose
+            v0, n0 = _map3(self.vertex_pyramid_t1[level], "vertex_t1"), _map3(self.normal_pyramid_t1[level], "normal_t1")
+            v1, n1 = _map3(self.vertex_pyramid_t0[level], "vertex_t0"), _map3(self.normal_pyramid_t0[level], "normal_t0")
+            if (tuple(self.intensity_pyramid_t1[level].shape) != tuple(v0.shape[:2])
+                    or tuple(self.intensity_pyramid_t0[level].shape) != tuple(v1.shape[:2])):
+                raise ValueError("colour and depth of a frame must have the same size")
+            keep += [v0, n0, v1, n1]
+            trk = self.icp_trackers[level]
+            e = lv[level]
+            e.vertex0, e.normal0, e.vertex1, e.normal1 = v0.data_ptr(), n0.data_ptr(), v1.data_ptr(), n1.data_ptr()
+            e.H, e.W = v0.shape[0], v0.shape[1]
+            e.fx, e.fy, e.cx, e.cy = (float(np.float32(k) * s) for k in Kf)
+            e.iters = int(trk.max_iterations)
+        t0 = self.icp_trackers[0]
+        out, pinned, event = _result_buffers_rgbd(device)
+        v_t0, v_t1, n_t0 = keep[-2], keep[-4], keep[-1]
+        H, W = v_t0.shape[:2]
+        stream = torch.cuda.current_stream(device)
+        check(L.rtg_icp_predict_pose_rgbd(lv, i0, i1, levels, float(t0.distance_threshold), float(t0.normal_threshold),
+                                          float(t0.damping), self.photometric_weight, None, _p(v_t0), _p(v_t1), _p(n_t0), H, W,
+                                          _p(out), C.c_void_p(pinned.data_ptr()), _p(_workspace(device)),
+                                          C.c_void_p(stream.cuda_stream)), "rtg_icp_predict_pose_rgbd")
+        event.record(stream)
+        event.synchronize()  # the kernel wrote the 20 floats into pinned host memory itself
+        host = pinned.numpy().copy()
+        pose_t1_t0 = host[:16].reshape(4, 4).astype(np.float32)
+        self.last_p2ploss, self.last_valid_ratio = float(host[16]), float(host[17])
+        self.last_photometric_ratio, self.last_photometric_rmse = float(host[18]), float(host[19])
+        if self.verbose:
+            print(self.last_p2ploss, self.last_valid_ratio, self.last_photometric_ratio, self.last_photometric_rmse)
         tracking_success = not (self.last_p2ploss > self.icp_fail_threshold)
         return pose_t1_t0, tracking_success

@@ -342,3 +342,56 @@ def raycast_room_depth(cam: Camera, box=(6.0, 3.0, 6.0), noise_sigma: float = 0.
         depth = depth + np.random.default_rng(seed).normal(0, noise_sigma, depth.shape)
     depth = np.where((depth < 0.3) | (depth > 5.0), 0.0, depth)
     return depth.astype(np.float32)
+
+
+def raycast_room_rgbd(cam: Camera, box=(6.0, 3.0, 6.0), noise_sigma: float = 0.0, seed: int = 3, spheres=DEFAULT_SPHERES,
+                      color_seed: int = 7, n_waves: int = 4):
+    """(depth (H,W) float32, colour (H,W,3) float32 in [0, 1]) of the textured box room seen from `cam.c2w`.
+
+    The depth is `raycast_room_depth`'s (same box, spheres, noise and range mask). The colour is a smooth function of the
+    world point the pixel's ray hits, so it moves with the scene, not with the camera: per channel 0.5 plus `n_waves`
+    sinusoids of seeded direction, phase, amplitude and wavelength (0.1 - 0.5 m), clipped to [0, 1]. `spheres=()` with the
+    camera facing a wall gives a planar view with texture. Pixels without depth take the colour at the camera centre."""
+    depth = raycast_room_depth(cam, box, noise_sigma, seed, spheres)
+    hit_z = raycast_room_depth(cam, box, 0.0, seed, spheres).astype(np.float64)
+    H, W = cam.height, cam.width
+    j, i = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
+    d_c = np.stack([(i - cam.cx) / cam.fx, (j - cam.cy) / cam.fy, np.ones_like(i, dtype=np.float64)], -1)
+    p_w = (d_c * hit_z[..., None]) @ cam.c2w[:3, :3].T + cam.c2w[:3, 3]
+    rng = np.random.default_rng(color_seed)
+    color = np.full((H, W, 3), 0.5)
+    for ch in range(3):
+        for _ in range(n_waves):
+            d = rng.normal(size=3)
+            d /= np.linalg.norm(d)
+            lam = rng.uniform(0.1, 0.5)
+            amp = rng.uniform(0.05, 0.15)
+            phase = rng.uniform(0, 2 * np.pi)
+            color[..., ch] += amp * np.sin(2 * np.pi * (p_w @ d) / lam + phase)
+    return depth, np.clip(color, 0.0, 1.0).astype(np.float32)
+
+
+def wall_cameras(W: int, H: int, dx: float = 0.02, dy: float = 0.015, deg: float = 1.0):
+    """Two cameras (TUM intrinsics scaled to width W) facing the room's far wall (z = 3 m) at 20 degrees, 1.1-2.1 m
+    away, with no other surface in view; the second is moved by (dx, dy) in the wall's plane and turned by `deg` about the
+    wall normal, the three directions a point-to-plane residual cannot see. Returns (cam0, cam1, ground-truth pose of
+    frame 1 in frame 0, i.e. cam0.w2c @ cam1.c2w)."""
+    s = W / 640.0
+    a, b = math.radians(20.0), math.radians(deg)
+    C0 = np.eye(4)
+    C0[:3, :3] = [[math.cos(a), 0, math.sin(a)], [0, 1, 0], [-math.sin(a), 0, math.cos(a)]]
+    C0[:3, 3] = (-0.5, 0.0, 1.5)
+    Rz = np.array([[math.cos(b), -math.sin(b), 0], [math.sin(b), math.cos(b), 0], [0, 0, 1]])
+    C1 = C0.copy()
+    C1[:3, :3] = Rz @ C0[:3, :3]
+    C1[:3, 3] = C0[:3, 3] + (dx, dy, 0.0)
+    cams = [Camera(W, H, 517.3 * s, 516.5 * s, 318.6 * s, 255.3 * s, c2w=c) for c in (C0, C1)]
+    return cams[0], cams[1], np.linalg.inv(C0) @ C1
+
+
+def wall_in_plane_error(cam0: Camera, cam1: Camera, pose) -> tuple:
+    """(in-plane translation error in m, rotation error about the wall normal in degrees) of a tracked pose of frame 1
+    in frame 0 on the views of `wall_cameras`."""
+    Ce = cam0.c2w @ np.asarray(pose, dtype=np.float64)
+    E = Ce @ np.linalg.inv(cam1.c2w)
+    return float(np.linalg.norm(Ce[:2, 3] - cam1.c2w[:2, 3])), abs(math.degrees(math.atan2(E[1, 0], E[0, 0])))

@@ -388,6 +388,35 @@ int rtg_splat_pose_gn_step_exposure(const RtgSplatView *view, int32_t P, int32_t
                                     int64_t R_cap, const int32_t *counters, const RtgPoseGN *s, const RtgPoseRobust *robust,
                                     const RtgPoseExposure *exposure, void *stream);
 
+/* Expected depth. With the pairs the forward blends (positions < n_contrib of the tile list, alpha past 1/255, the
+ * forward's own decisions), w_i = alpha_i T_i and z_i the view-space z of Gaussian i's centre, per pixel
+ *   m1 = sum w_i (coverage),  m0 = sum w_i z_i,  D = m0 / m1 (0 where m1 = 0),
+ * the map rtg_splat_features composites for F = (z_view, 1), summed in the same order. Its tangents, with dz_i/dxi =
+ * (0, 0, 1, p_y, -p_x, 0): dm1 = sum dw_i, dm0 = sum (dw_i z_i + w_i dz_i), dD = (dm0 - D dm1) / m1.
+ *
+ * rtg_splat_pose_tangents_expected: rtg_splat_pose_tangents with dD/dxi_k in channel 3 of J (0 where m1 = 0), and
+ * `expected` (2, H, W) fp32 = (D, m1), both written everywhere (0 in a never-rendered or masked-out tile). It takes no
+ * hit map. `scratch` holds rtg_splat_pose_gn_scratch_bytes(P, H, W) bytes. Validates on the host before any CUDA work. */
+int rtg_splat_pose_tangents_expected(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                                     const float *colors_precomp, const float *scales, const float *rotations,
+                                     const float *cov3D_precomp, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                                     int64_t R_cap, const int32_t *counters, void *scratch, float *J, float *expected,
+                                     void *stream);
+
+/* rtg_splat_pose_gn_step_expected: the step of rtg_splat_pose_gn_step[_robust|_exposure] with the expected depth in place
+ * of the hit depth. The depth residual is D - D^ over S_e: in the render mask, m1 >= min_coverage, gt_depth > 0 and
+ * D - gt_depth < depth_error_max (signed); N_d = |S_e|. The colour rows, the weights, the Huber rule, the objective, the
+ * damping, the solve, the update and the report are those of the entry point the arguments select: `robust->kernel`
+ * RTG_ROBUST_NONE or RTG_ROBUST_HUBER, and `exposure` NULL (six unknowns, scratch rtg_splat_pose_gn_scratch_bytes) or
+ * the device exposure (eight unknowns, scratch rtg_splat_pose_gn_exposure_scratch_bytes). `s->depth` and `s->hit_depth`
+ * are validated as there but not read. Rejects min_coverage outside (0, 1], a NULL `robust`, a NULL or misaligned
+ * `exposure->ab` and everything rtg_splat_pose_gn_step_robust rejects, on the host before any CUDA work. */
+int rtg_splat_pose_gn_step_expected(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                                    const float *colors_precomp, const float *scales, const float *rotations,
+                                    const float *cov3D_precomp, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                                    int64_t R_cap, const int32_t *counters, const RtgPoseGN *s, const RtgPoseRobust *robust,
+                                    const RtgPoseExposure *exposure, float min_coverage, void *stream);
+
 /* ---- per-Gaussian contributions to a frame (no reference counterpart) ----------------------------------------------
  * rtg_splat_contributions: what each Gaussian added to the render of one rtg_splat_forward (its view, workspaces, R_cap
  * and counters; the view's flags must be the forward's). The pairs (p, g) that add colour are those the forward blends and

@@ -150,6 +150,12 @@ SIGNATURES = {
     "rtg_splat_pose_gn_exposure_scratch_bytes": (C.c_size_t, [_I32, _I32, _I32]),
     "rtg_splat_pose_gn_step_exposure": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
                                         + [C.POINTER(RtgPoseGN), C.POINTER(RtgPoseRobust), C.POINTER(RtgPoseExposure), _VP]),
+    # view, P, M, 6 Gaussian inputs, 3 workspaces, R_cap, counters, scratch, J, expected, stream
+    "rtg_splat_pose_tangents_expected": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
+                                         + [_VP] * 4),
+    "rtg_splat_pose_gn_step_expected": (C.c_int, [C.POINTER(RtgSplatView), _I32, _I32] + [_VP] * 6 + [_VP] * 3 + [_I64, _VP]
+                                        + [C.POINTER(RtgPoseGN), C.POINTER(RtgPoseRobust), C.POINTER(RtgPoseExposure), _F,
+                                           _VP]),
     "rtg_splat_mark_visible": (C.c_int, [_I32, _VP, _VP, _VP, _VP, _VP]),
     "rtg_adam_step": (C.c_int, [C.POINTER(RtgAdamGroup), _I32, _F, _F, _F, _I32, _VP]),
     "rtg_map_adam_step": (C.c_int, [C.POINTER(RtgMapStep), _VP]),

@@ -20,6 +20,9 @@ void launch_pose_gn_normal_eq_step(const ViewParams &vp, int P, const GeomState 
 void launch_pose_gn_exposure_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
                                   const int32_t *counters, const RtgPoseGN &st, const RtgPoseRobust &robust, double *ab,
                                   cudaStream_t s);
+void launch_pose_gn_expected_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                  const int32_t *counters, const RtgPoseGN &st, const RtgPoseRobust &robust, double *ab,
+                                  float min_cov, cudaStream_t s);
 void launch_frame_downsample(const float *color, const float *depth, const uint8_t *render_mask, const int32_t *tile_mask, int H,
                              int W, int scale, int channels_last, float *color_out, float *depth_out, uint8_t *mask_out,
                              int32_t *tile_mask_out, cudaStream_t s);
@@ -540,12 +543,13 @@ size_t rtg_splat_pose_gn_scratch_bytes(int32_t P, int32_t H, int32_t W) {
 static int validate_pose_tangent_inputs(const char *who, const RtgSplatView *view, int32_t P, int32_t M, const float *means3D,
                                         const float *shs, const float *colors_precomp, const float *scales, const float *rotations,
                                         const float *cov3D_precomp, const void *geom_ws, const void *img_ws, const void *bin_ws,
-                                        int64_t R_cap, const int32_t *counters, const int32_t *hit_image, const void *scratch) {
+                                        int64_t R_cap, const int32_t *counters, const int32_t *hit_image, const void *scratch,
+                                        bool need_hit = true) {
     int rc = validate_view(view, who);
     if (rc) return rc;
     if (P < 1) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": P must be >= 1");
     if (R_cap < 0) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": R_cap < 0");
-    if (!means3D || !geom_ws || !img_ws || !bin_ws || !counters || !hit_image || !scratch)
+    if (!means3D || !geom_ws || !img_ws || !bin_ws || !counters || (need_hit && !hit_image) || !scratch)
         return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pointer");
     if ((shs == nullptr) == (colors_precomp == nullptr))
         return fail(RTG_ERR_INVALID_ARGUMENT, "Please provide excatly one of either SHs or precomputed colors!");
@@ -577,6 +581,30 @@ int rtg_splat_pose_tangents(const RtgSplatView *view, int32_t P, int32_t M, cons
     rtg::launch_preprocess_tangent(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count,
                                    reinterpret_cast<float4 *>(scratch), s);
     rtg::launch_render_tangent_images(vp, P, g, b, img, counters, hit_image, scratch, J, s);
+    return check_launch(who);
+}
+
+int rtg_splat_pose_tangents_expected(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                                     const float *colors_precomp, const float *scales, const float *rotations,
+                                     const float *cov3D_precomp, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                                     int64_t R_cap, const int32_t *counters, void *scratch, float *J, float *expected,
+                                     void *stream) {
+    const char *who = "rtg_splat_pose_tangents_expected";
+    int rc = validate_pose_tangent_inputs(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws,
+                                          img_ws, bin_ws, R_cap, counters, nullptr, scratch, false);
+    if (rc) return rc;
+    if (!J || !expected) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": J / expected is NULL");
+    if ((((uintptr_t)J) | ((uintptr_t)expected)) & 3)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": J / expected must be 4-byte aligned");
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const rtg::ViewParams vp = make_view(view);
+    const int T = vp.tiles_x * vp.tiles_y;
+    rtg::GeomState g = rtg::geom_from(const_cast<void *>(geom_ws), (size_t)P);
+    rtg::ImgState img = rtg::img_from(const_cast<void *>(img_ws), (size_t)vp.H * vp.W);
+    rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
+    rtg::launch_preprocess_tangent(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count,
+                                   reinterpret_cast<float4 *>(scratch), s);
+    rtg::launch_render_tangent_expected_images(vp, P, g, b, img, counters, scratch, J, expected, s);
     return check_launch(who);
 }
 
@@ -737,11 +765,12 @@ int rtg_splat_features_backward_geometry(const RtgSplatView *view, int32_t P, co
 }
 
 // The step of the Gauss-Newton entry points: `robust` selects the normal-equation rows (RTG_ROBUST_NONE: the plain ones),
-// `ab` (the device exposure, or nullptr) the eight-unknown step.
+// `ab` (the device exposure, or nullptr) the eight-unknown step, `expected` the expected-depth residual on S_e(min_cov).
 static int pose_gn_step(const char *who, const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
                         const float *colors_precomp, const float *scales, const float *rotations, const float *cov3D_precomp,
                         const void *geom_ws, const void *img_ws, const void *bin_ws, int64_t R_cap, const int32_t *counters,
-                        const RtgPoseGN *st, const RtgPoseRobust &robust, double *ab, void *stream) {
+                        const RtgPoseGN *st, const RtgPoseRobust &robust, double *ab, void *stream, bool expected = false,
+                        float min_cov = 0.f) {
     int rc = validate_pose_tangent_inputs(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws,
                                           img_ws, bin_ws, R_cap, counters, st->hit_depth, st->scratch);
     if (rc) return rc;
@@ -761,7 +790,8 @@ static int pose_gn_step(const char *who, const RtgSplatView *view, int32_t P, in
     rtg::BinState b = rtg::bin_from(const_cast<void *>(bin_ws), (size_t)T, (size_t)R_cap);
     rtg::launch_preprocess_tangent(vp, P, M, means3D, scales, rotations, shs, cov3D_precomp, g, b.vis_count,
                                    reinterpret_cast<float4 *>(st->scratch), s);
-    if (ab) rtg::launch_pose_gn_exposure_step(vp, P, g, b, img, counters, *st, robust, ab, s);
+    if (expected) rtg::launch_pose_gn_expected_step(vp, P, g, b, img, counters, *st, robust, ab, min_cov, s);
+    else if (ab) rtg::launch_pose_gn_exposure_step(vp, P, g, b, img, counters, *st, robust, ab, s);
     else rtg::launch_pose_gn_normal_eq_step(vp, P, g, b, img, counters, *st, robust, s);
     return check_launch(who);
 }
@@ -817,6 +847,27 @@ int rtg_splat_pose_gn_step_exposure(const RtgSplatView *view, int32_t P, int32_t
     if (((uintptr_t)exposure->ab) & 7) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": exposure ab must be 8-byte aligned");
     return pose_gn_step(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws, img_ws, bin_ws,
                         R_cap, counters, st, *robust, exposure->ab, stream);
+}
+
+int rtg_splat_pose_gn_step_expected(const RtgSplatView *view, int32_t P, int32_t M, const float *means3D, const float *shs,
+                                    const float *colors_precomp, const float *scales, const float *rotations,
+                                    const float *cov3D_precomp, const void *geom_ws, const void *img_ws, const void *bin_ws,
+                                    int64_t R_cap, const int32_t *counters, const RtgPoseGN *st, const RtgPoseRobust *robust,
+                                    const RtgPoseExposure *exposure, float min_coverage, void *stream) {
+    const char *who = "rtg_splat_pose_gn_step_expected";
+    int rc = validate_pose_robust(who, st, robust);
+    if (rc) return rc;
+    if (!(min_coverage > 0.f && min_coverage <= 1.f))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": min_coverage must be in (0, 1]");
+    double *ab = nullptr;
+    if (exposure) {
+        if (!exposure->ab) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": exposure ab is NULL");
+        if (((uintptr_t)exposure->ab) & 7)
+            return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": exposure ab must be 8-byte aligned");
+        ab = exposure->ab;
+    }
+    return pose_gn_step(who, view, P, M, means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, geom_ws, img_ws, bin_ws,
+                        R_cap, counters, st, *robust, ab, stream, true, min_coverage);
 }
 
 int rtg_pose_adam_step(const RtgPoseAdam *st, void *stream) {

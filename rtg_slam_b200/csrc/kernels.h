@@ -56,6 +56,9 @@ size_t pose_gn_scratch_bytes(int P, int H, int W);
 size_t pose_gn_exposure_scratch_bytes(int P, int H, int W);  // the per-tile rows hold RTG_GN_EXP_ALL terms
 void launch_render_tangent_images(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
                                   const int32_t *counters, const int *hit_image, void *scratch, float *J, cudaStream_t s);
+// the same with the expected depth in channel 3 of J, and its (D, m1) map in `expected` (2, H, W)
+void launch_render_tangent_expected_images(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                           const int32_t *counters, void *scratch, float *J, float *expected, cudaStream_t s);
 // per-Gaussian pixel counts, weight sums and (pixel_error != NULL) weighted error of the forward, added into the outputs
 void launch_render_contributions(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
                                  const int32_t *counters, const float *pixel_error, int32_t *n_pixels, float *weight, float *error,

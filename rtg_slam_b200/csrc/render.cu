@@ -792,11 +792,18 @@ __device__ __forceinline__ float huber_weight(const float r, const float delta) 
 
 // The body of the kernel signatures below; `huber` (colour, depth thresholds) is read by the robust modes only and `ab`
 // (the device exposure) by the exposure modes only.
-template <int MODE, bool AA>
+// ED (expected depth) replaces the hit depth by the alpha-blended depth of the same pairs: with w_i = alpha_i T_i and z_i
+// the view-space z of Gaussian i's centre (hit record), m1 = sum w_i, m0 = sum w_i z_i, D = m0 / m1 (0 where m1 = 0) and
+//   dz_i = (0, 0, 1, p_y, -p_x, 0),  dm1 = sum dw_i,  dm0 = sum (dw_i z_i + w_i dz_i),  dD = (dm0 - D dm1) / m1,
+// carried in place of the hit-depth tangent. dT_{i+1} = dT_i - dw_i, so the sum telescopes to dm1 = -dT_final: the replay
+// carries m0, m1 and dm0 only (m1 itself is summed, in render_feat_fwd_kernel's order, so that it is that map's coverage). TAN_IMAGES also writes (D, m1) to `expected` (2, H, W); the normal-equation
+// modes take the depth residual D - D^ on S_e: in the mask, m1 >= min_cov, gt_depth > 0, D - gt_depth < depth_error_max.
+template <int MODE, bool AA, bool ED = false>
 __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
                                                     const int *__restrict__ counters, const int *__restrict__ hit_image,
                                                     const float4 *__restrict__ tan, float *__restrict__ J, const GnInputs &in,
-                                                    const float2 huber, const double *__restrict__ ab) {
+                                                    const float2 huber, const double *__restrict__ ab,
+                                                    float *__restrict__ expected = nullptr, const float min_cov = 0.f) {
     constexpr bool EXPOSURE = tan_exposure(MODE);
     constexpr int NT = EXPOSURE ? RTG_GN_EXP_ALL : RTG_GN_ALL;
     __shared__ float4 s_s0[BATCH], s_s1[BATCH], s_rgb[BATCH];
@@ -831,6 +838,10 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
     float T = 1.f, dT[6], dC[3][6];
 #pragma unroll
     for (int k = 0; k < 6; k++) { dT[k] = 0.f; dC[0][k] = dC[1][k] = dC[2][k] = 0.f; }
+    [[maybe_unused]] float m0 = 0.f, m1 = 0.f, dm0[6];
+    if constexpr (ED)
+#pragma unroll
+        for (int k = 0; k < 6; k++) dm0[k] = 0.f;
 
     const int rounds = ((int)m + BATCH - 1) / BATCH;
     for (int i = 0; i < rounds; i++) {
@@ -877,6 +888,8 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
                             dlc[k] = tr_k.y; dlc[k + 3] = tr_k.z;
                         }
                     }
+                    [[maybe_unused]] float4 pc;  // ED: the view-space centre (x, y, z) of the hit record
+                    if constexpr (ED) pc = __ldg(g.hit + 2 * (size_t)s_id[j] + 1);
 #pragma unroll
                     for (int k = 0; k < 6; k++) {
                         const float4 ta = __ldg(tr + 2 * k);
@@ -888,7 +901,18 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
                         dC[0][k] += tb.y * wgt + col.x * dw;
                         dC[1][k] += tb.z * wgt + col.y * dw;
                         dC[2][k] += tb.w * wgt + col.z * dw;
+                        if constexpr (ED) {
+                            float dm = dw * pc.z;  // + w dz, dz = (0, 0, 1, p_y, -p_x, 0)
+                            if (k == 2) dm += wgt;
+                            if (k == 3) dm += wgt * pc.y;
+                            if (k == 4) dm -= wgt * pc.x;
+                            dm0[k] += dm;
+                        }
                         dT[k] = dT[k] * (1.f - alpha) - T * dal;
+                    }
+                    if constexpr (ED) {  // in the order and form of render_feat_fwd_kernel's F = (z, 1) accumulators
+                        m0 += wgt * pc.z;
+                        m1 += wgt;
                     }
                     T = T * (1.f - alpha);
                 }
@@ -901,7 +925,16 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
 #pragma unroll
     for (int k = 0; k < 6; k++) { dC[0][k] += bg0 * dT[k]; dC[1][k] += bg1 * dT[k]; dC[2][k] += bg2 * dT[k]; }
     float dD[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    const int gid = (inside && n > 0) ? hit_image[pix] : -1;  // a never-rendered tile's hit map holds 0, not a hit
+    [[maybe_unused]] float D = 0.f;  // ED: the expected depth
+    if constexpr (ED) {
+        if (m1 > 0.f) {
+            D = m0 / m1;
+            const float inv = 1.f / m1;
+#pragma unroll
+            for (int k = 0; k < 6; k++) dD[k] = (dm0[k] + D * dT[k]) * inv;  // dm1 = -dT
+        }
+    }
+    const int gid = (!ED && inside && n > 0) ? hit_image[pix] : -1;  // a never-rendered tile's hit map holds 0, not a hit
     if (gid >= 0) {
         const float3 ray = pixel_ray(px, py, vp.focal_x, vp.focal_y, vp.cx, vp.cy);
         const float4 h0 = __ldg(g.hit + 2 * (size_t)gid), h1 = __ldg(g.hit + 2 * (size_t)gid + 1);
@@ -929,6 +962,7 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
                 float *o = J + (size_t)(4 * k) * HW + pix;
                 o[0] = dC[0][k]; o[HW] = dC[1][k]; o[2 * HW] = dC[2][k]; o[3 * HW] = dD[k];
             }
+            if constexpr (ED) { expected[pix] = D; expected[HW + pix] = m1; }
         }
     } else {
         const int N = vp.H * vp.W;
@@ -947,8 +981,13 @@ __device__ __forceinline__ void render_tangent_body(const ViewParams &vp, const 
                 }
             }
             const float gd = in.gt_depth[pix];
-            rd = in.depth[pix] - gd;
-            sd = frame_depth_pixel(hit_image[pix], gd, rd, in.depth_error_max);  // rtg_loss_l1's depth pixels
+            if constexpr (ED) {
+                rd = D - gd;
+                sd = m1 >= min_cov && gd > 0.f && rd < in.depth_error_max;  // S_e
+            } else {
+                rd = in.depth[pix] - gd;
+                sd = frame_depth_pixel(hit_image[pix], gd, rd, in.depth_error_max);  // rtg_loss_l1's depth pixels
+            }
         }
         if constexpr (EXPOSURE) {
             // Each term is reduced as soon as it is formed (double warp butterfly, lane 0 stores the warp's sum), the depth
@@ -1074,6 +1113,16 @@ __global__ void __launch_bounds__(256, 2) render_tangent_kernel(const ViewParams
                                                              const float2 huber, const double *__restrict__ ab) {
     static_assert(tan_exposure(MODE), "only the exposure rows read the device exposure");
     render_tangent_body<MODE, AA>(vp, g, b, img, counters, hit_image, tan, J, in, huber, ab);
+}
+// Every mode with the expected depth in place of the hit depth (one signature: the unused arguments are not read), at two
+// CTAs per SM: without the bound the normal-equation modes take 152 registers, one CTA.
+template <int MODE, bool AA>
+__global__ void __launch_bounds__(256, 2)
+    render_tangent_expected_kernel(const ViewParams vp, const GeomState g, const BinState b, const ImgState img,
+                                   const int *__restrict__ counters, const float4 *__restrict__ tan, float *__restrict__ J,
+                                   const GnInputs in, const float2 huber, const double *__restrict__ ab,
+                                   float *__restrict__ expected, const float min_cov) {
+    render_tangent_body<MODE, AA, true>(vp, g, b, img, counters, nullptr, tan, J, in, huber, ab, expected, min_cov);
 }
 
 // One block: the fixed-order sum of the tiles' rows (one warp per term, fixed lane stride, fixed butterfly), then on one
@@ -1262,6 +1311,48 @@ void launch_pose_gn_exposure_step(const ViewParams &vp, int P, const GeomState &
     else
         render_tangent_kernel<TAN_NORMAL_EQ_EXPOSURE, false><<<T, 256, 0, s>>>(vp, g, b, img, counters, st.hit_depth, tan, nullptr, in, huber, ab);
     pose_gn_exposure_step_kernel<<<1, 256, 0, s>>>(T, in.partial, counters, st, ab);
+}
+
+void launch_render_tangent_expected_images(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                           const int32_t *counters, void *scratch, float *J, float *expected, cudaStream_t s) {
+    const int T = vp.tiles_x * vp.tiles_y;
+    const float4 *tan = tan_rows(scratch);
+    const float2 h = make_float2(0.f, 0.f);
+    if (vp.antialiased)
+        render_tangent_expected_kernel<TAN_IMAGES, true><<<T, 256, 0, s>>>(vp, g, b, img, counters, tan, J, GnInputs{}, h, nullptr, expected, 0.f);
+    else
+        render_tangent_expected_kernel<TAN_IMAGES, false><<<T, 256, 0, s>>>(vp, g, b, img, counters, tan, J, GnInputs{}, h, nullptr, expected, 0.f);
+}
+
+template <int MODE>
+static void launch_tangent_expected_rows(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img,
+                                         const int32_t *counters, const float4 *tan, const GnInputs &in, const float2 huber,
+                                         const double *ab, const float min_cov, cudaStream_t s) {
+    const int T = vp.tiles_x * vp.tiles_y;
+    if (vp.antialiased)
+        render_tangent_expected_kernel<MODE, true><<<T, 256, 0, s>>>(vp, g, b, img, counters, tan, nullptr, in, huber, ab, nullptr, min_cov);
+    else
+        render_tangent_expected_kernel<MODE, false><<<T, 256, 0, s>>>(vp, g, b, img, counters, tan, nullptr, in, huber, ab, nullptr, min_cov);
+}
+
+void launch_pose_gn_expected_step(const ViewParams &vp, int P, const GeomState &g, const BinState &b, const ImgState &img,
+                                  const int32_t *counters, const RtgPoseGN &st, const RtgPoseRobust &robust, double *ab,
+                                  float min_cov, cudaStream_t s) {
+    const int T = vp.tiles_x * vp.tiles_y;
+    GnInputs in{st.render, st.depth, st.gt_color, st.gt_depth, st.render_mask, st.gt_channels_last, st.depth_error_max,
+                gn_partial(st.scratch, P)};
+    const float2 huber = make_float2(robust.color_delta, robust.depth_delta);
+    const float4 *tan = tan_rows(st.scratch);
+    const bool hub = robust.kernel == RTG_ROBUST_HUBER;
+    if (ab) {
+        if (hub) launch_tangent_expected_rows<TAN_NORMAL_EQ_EXPOSURE_ROBUST>(vp, g, b, img, counters, tan, in, huber, ab, min_cov, s);
+        else launch_tangent_expected_rows<TAN_NORMAL_EQ_EXPOSURE>(vp, g, b, img, counters, tan, in, huber, ab, min_cov, s);
+        pose_gn_exposure_step_kernel<<<1, 256, 0, s>>>(T, in.partial, counters, st, ab);
+    } else {
+        if (hub) launch_tangent_expected_rows<TAN_NORMAL_EQ_ROBUST>(vp, g, b, img, counters, tan, in, huber, nullptr, min_cov, s);
+        else launch_tangent_expected_rows<TAN_NORMAL_EQ>(vp, g, b, img, counters, tan, in, huber, nullptr, min_cov, s);
+        pose_gn_step_kernel<<<1, 256, 0, s>>>(T, in.partial, counters, st);
+    }
 }
 
 void launch_render_fwd(const ViewParams &vp, const GeomState &g, const BinState &b, const ImgState &img, const int32_t *counters,

@@ -58,12 +58,21 @@ def _native_args(rs, saved, ins, dev):
             saved.r_cap, C.c_void_p(saved.counters))
 
 
+def _check_depth(depth):
+    if depth not in ("hit", "expected"):
+        raise ValueError('depth must be "hit" or "expected"')
+
+
 def pose_jacobian(raster_settings, means3D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                  cov3D_precomp=None, tile_mask=None):
+                  cov3D_precomp=None, tile_mask=None, depth="hit"):
     """One rasterizer forward at the settings' camera and the forward-mode tangents of its render along the six directions
     of a left twist xi = (rho, phi) of the pose (rtg_splat_pose_tangents). Returns (outputs, J): the forward's eight outputs
     as GaussianRasterizer returns them, and J (6, 4, H, W) float32, J[k] = d(colour r, g, b, depth) / d xi_k. Inputs as
-    GaussianRasterizer takes them; nothing is differentiated by autograd."""
+    GaussianRasterizer takes them; nothing is differentiated by autograd.
+    `depth="expected"` (rtg_splat_pose_tangents_expected): channel 3 of J is the tangent of the alpha-blended depth
+    D = sum w z / sum w of the forward's blend weights w = alpha T (0 where sum w = 0), and a third value is returned:
+    `expected` (2, H, W) float32 = (D, sum w), the map the tangents were replayed from."""
+    _check_depth(depth)
     with torch.no_grad():
         dev = means3D.device
         st = rasterizer._state(dev)
@@ -80,6 +89,13 @@ def pose_jacobian(raster_settings, means3D, opacities, shs=None, colors_precomp=
         P = int(means3D.shape[0])
         scratch = torch.empty((int(L.rtg_splat_pose_gn_scratch_bytes(P, H, W)),), dtype=torch.uint8, device=dev)
         J = torch.empty((6, 4, H, W), dtype=torch.float32, device=dev)
+        if depth == "expected":
+            expected = torch.empty((2, H, W), dtype=torch.float32, device=dev)
+            check(L.rtg_splat_pose_tangents_expected(*_native_args(raster_settings, saved, ins, dev), C.c_void_p(scratch.data_ptr()),
+                                                     C.c_void_p(J.data_ptr()), C.c_void_p(expected.data_ptr()),
+                                                     C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                  "rtg_splat_pose_tangents_expected")
+            return outs, J, expected
         check(L.rtg_splat_pose_tangents(*_native_args(raster_settings, saved, ins, dev), C.c_void_p(outs[3].data_ptr()),
                                         C.c_void_p(scratch.data_ptr()), C.c_void_p(J.data_ptr()),
                                         C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "rtg_splat_pose_tangents")
@@ -190,7 +206,7 @@ class PoseRefiner:
 
     def refine_gn(self, camera, gaussian_data, gt_color, gt_depth, iters, damping=1e-4, color_weight=0.8, depth_weight=1.0,
                   render_mask=None, tile_mask=None, depth_error_max=0.1, scales=(1,), robust=None, color_delta=0.1,
-                  depth_delta=0.05, exposure=None, coarse_antialias=False):
+                  depth_delta=0.05, exposure=None, coarse_antialias=False, depth="hit", min_coverage=0.5):
         """Gauss-Newton refinement of the pose on the squared colour + depth residuals (rtg_splat_pose_gn_step): per
         iteration the rasterizer forward, then the forward-mode tangents of the render along the six twist directions, the
         normal equations over rtg_loss_l1's pixel selection, the damped solve (H + damping * trace(H) * I) and
@@ -215,6 +231,11 @@ class PoseRefiner:
         `coarse_antialias`: True renders the levels s >= 2 antialiased (`rasterizer.antialiased`): a map of sub-pixel
         surfels then renders at a coarse level close to the block mean of its fine render, which a plain render is not.
         Level 1 renders in the mode of the caller's context.
+        `depth`: "hit" (the default) takes the depth residual on the opaque-surfel depth of the pixel's hit Gaussian, as
+        above. "expected" (rtg_splat_pose_gn_step_expected) takes it on the alpha-blended depth D = sum w z / sum w of the
+        forward's blend weights w = alpha T, over the pixels of the render mask with coverage sum w >= `min_coverage` (in
+        (0, 1]), a measured depth and D - gt_depth < depth_error_max; the colour rows, weights, Huber rule and exposure are
+        unchanged. It combines with `scales`, `coarse_antialias`, `robust` and `exposure`.
 
         Returns (W2C, report): the refined pose, a (4, 4) float64 CUDA tensor, and the finest level's last step's report,
         a float64 CUDA tensor [E, E_colour, E_depth, N_c, N_d, |rho|, |phi|, status] (E evaluated before that step; status
@@ -229,6 +250,10 @@ class PoseRefiner:
             raise ValueError("iters must be >= 1")
         if robust not in (None, "huber"):
             raise ValueError('robust must be None or "huber"')
+        _check_depth(depth)
+        min_coverage = float(min_coverage)
+        if not 0.0 < min_coverage <= 1.0:
+            raise ValueError("min_coverage must be in (0, 1]")
         dev, pose, projection, view, proj, campos, rs, g = self._setup(camera, gaussian_data, requires_grad=False)
         H, W = int(rs.image_height), int(rs.image_width)
         gt_color, gt_depth, mask, channels_last = frame_targets(gt_color, gt_depth, render_mask, H, W)
@@ -266,6 +291,10 @@ class PoseRefiner:
             ab = _exposure_pair(exposure, dev, torch.float64)
             ex = _lib.RtgPoseExposure()
             ex.ab = ab.data_ptr()
+        if depth == "expected":  # one entry point for every combination
+            step = L.rtg_splat_pose_gn_step_expected
+            extra = (C.byref(r), None if exposure is None else C.byref(ex), min_coverage)
+        elif exposure is not None:
             step, extra = L.rtg_splat_pose_gn_step_exposure, (C.byref(r), C.byref(ex))
         elif robust is None:
             step, extra = L.rtg_splat_pose_gn_step, ()

@@ -683,6 +683,20 @@ int rtg_loss_mapping(const float *render, const float *depth, const float *rende
                      int32_t gt_channels_last, float color_weight, float depth_weight, float normal_weight, float depth_error_max,
                      float *dL_dcolor, float *dL_ddepth, float *dL_dnormal, float *loss_out, void *ws, void *stream);
 
+/* rtg_loss_mapping_exposure: rtg_loss_mapping of a render seen under an exposure (a, b) = `exposure` (2 device floats), as
+ * rtg_loss_l1_exposure is rtg_loss_l1's: the colour residual is r = e^a render + b - gt_color, the depth and normal terms are
+ * unchanged, and
+ *   dL_dcolor = color_weight / N_c e^a sgn(r),
+ *   dL_dexposure (2 device floats) = color_weight / N_c (sum sgn(r) e^a render, sum sgn(r)),  N_c = 3 x selected pixels.
+ * loss_out keeps rtg_loss_mapping's 8 floats. exposure = (0, 0) gives rtg_loss_mapping's loss_out and gradients bit for bit.
+ * Sums, workspace (rtg_loss_workspace_bytes()) and validation as rtg_loss_mapping; exposure and dL_dexposure must not be
+ * NULL. */
+int rtg_loss_mapping_exposure(const float *render, const float *depth, const float *render_normal, const int32_t *depth_index,
+                              const float *gt_color, const float *gt_depth, const float *gt_normal, const uint8_t *render_mask,
+                              int32_t H, int32_t W, int32_t gt_channels_last, float color_weight, float depth_weight,
+                              float normal_weight, float depth_error_max, const float *exposure, float *dL_dcolor, float *dL_ddepth,
+                              float *dL_dnormal, float *dL_dexposure, float *loss_out, void *ws, void *stream);
+
 /* SSIM term of Mapping.loss_update (mapper.py:411-415: ssim_loss = 1 - ssim(render, gt), evaluated only without a render
  * mask) with ssim of utils/loss_utils.py:40-100: 11x11 Gaussian window (sigma 1.5, one per channel), zero padding,
  * C1 = 0.01^2, C2 = 0.03^2, mean over all C*H*W entries of the ssim map. img1, img2: (C,H,W).
@@ -692,6 +706,17 @@ int rtg_loss_mapping(const float *render, const float *depth, const float *rende
 size_t rtg_ssim_workspace_bytes(int32_t C, int32_t H, int32_t W);
 int rtg_ssim_loss(const float *img1, const float *img2, int32_t C, int32_t H, int32_t W, float *dL_dimg1, float *loss_out, void *ws,
                   void *stream);
+
+/* rtg_ssim_loss_exposure: 1 - ssim(e^a img1 + b, img2) with (a, b) = `exposure` (2 device floats): img1 seen under the
+ * exposure, then rtg_ssim_loss. Written: loss_out as rtg_ssim_loss; dL_dimg1 (C,H,W) = e^a dL/dx^ with x^ = e^a img1 + b;
+ * dL_dexposure (2 device floats) = (sum dL/dx^ e^a img1, sum dL/dx^), from per-CTA double partials added in a fixed order
+ * (bit-reproducible). dL_dimg1 and dL_dexposure may each be NULL; with both NULL only the value is computed.
+ * ws: rtg_ssim_exposure_workspace_bytes(C, H, W) bytes (rtg_ssim_workspace_bytes plus the exposure partials), 8-byte
+ * aligned. Rejects NULL img1 / img2 / exposure / loss_out / ws, C outside [1, 65535], H or W < 1 and ceil(H / 16) > 65535
+ * on the host before any CUDA work. exposure = (0, 0) gives rtg_ssim_loss's loss_out and dL_dimg1 bit for bit. */
+size_t rtg_ssim_exposure_workspace_bytes(int32_t C, int32_t H, int32_t W);
+int rtg_ssim_loss_exposure(const float *img1, const float *img2, int32_t C, int32_t H, int32_t W, const float *exposure,
+                           float *dL_dimg1, float *dL_dexposure, float *loss_out, void *ws, void *stream);
 
 /* render_normal of Renderer.render (SLAM/render.py:130-133): out (3,H,W) = normal[depth_index] where the index is
  * > -1, zeros elsewhere; normal is (P,3). */

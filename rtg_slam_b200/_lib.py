@@ -179,8 +179,13 @@ SIGNATURES = {
     "rtg_loss_l1_exposure_workspace_bytes": (C.c_size_t, []),
     "rtg_loss_l1_exposure": (C.c_int, [_VP] * 6 + [_I32, _I32, _I32, _F, _F, _F, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "rtg_loss_mapping": (C.c_int, [_VP] * 8 + [_I32, _I32, _I32, _F, _F, _F, _F, _VP, _VP, _VP, _VP, _VP, _VP]),
+    # rtg_loss_mapping's arguments with exposure after depth_error_max and dL_dexposure after dL_dnormal
+    "rtg_loss_mapping_exposure": (C.c_int, [_VP] * 8 + [_I32, _I32, _I32, _F, _F, _F, _F, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "rtg_ssim_workspace_bytes": (C.c_size_t, [_I32, _I32, _I32]),
     "rtg_ssim_loss": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _VP, _VP, _VP, _VP]),
+    "rtg_ssim_exposure_workspace_bytes": (C.c_size_t, [_I32, _I32, _I32]),
+    # img1, img2, C, H, W, exposure, dL_dimg1, dL_dexposure, loss_out, ws, stream
+    "rtg_ssim_loss_exposure": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP]),
     "rtg_normal_map": (C.c_int, [_VP, _VP, _I32, _I32, _VP, _VP]),
     "rtg_frame_preprocess": (C.c_int, [_VP, _I32, _I32, _I32, _I32] + [_F] * 9 + [_VP] * 7),
     # color, depth, render_mask, tile_mask, H, W, scale, color_channels_last, 4 outputs, stream

@@ -53,6 +53,14 @@ void launch_loss_l1_exposure(const float *render, const float *depth, const int 
                              const float *gt_depth, const uint8_t *mask, int H, int W, int channels_last, float color_weight,
                              float depth_weight, float depth_error_max, const float *exposure, float *dL_dcolor, float *dL_ddepth,
                              float *dL_dexposure, float *loss_out, void *ws, cudaStream_t s);
+void launch_loss_mapping_exposure(const float *render, const float *depth, const float *render_normal, const int *depth_index,
+                                  const float *gt_color, const float *gt_depth, const float *gt_normal, const uint8_t *mask, int H,
+                                  int W, int channels_last, float color_weight, float depth_weight, float normal_weight,
+                                  float depth_error_max, const float *exposure, float *dL_dcolor, float *dL_ddepth,
+                                  float *dL_dnormal, float *dL_dexposure, float *loss_out, void *ws, cudaStream_t s);
+size_t ssim_exposure_ws_bytes(int C, int H, int W);
+void launch_ssim_loss_exposure(const float *img1, const float *img2, int C, int H, int W, const float *exposure, float *dL_dimg1,
+                               float *dL_dexposure, float *loss_out, void *ws, cudaStream_t s);
 void launch_normal_map(const float *normal, const int *depth_index, int H, int W, float *out, cudaStream_t s);
 void launch_icp_fill(float *render_depth, const float *frame_depth, const float *rn, const float *fn, int H, int W, float dthr,
                      float nthr, cudaStream_t s);
@@ -1149,6 +1157,23 @@ int rtg_loss_mapping(const float *render, const float *depth, const float *rende
     return check_launch(who);
 }
 
+int rtg_loss_mapping_exposure(const float *render, const float *depth, const float *render_normal, const int32_t *depth_index,
+                              const float *gt_color, const float *gt_depth, const float *gt_normal, const uint8_t *render_mask,
+                              int32_t H, int32_t W, int32_t gt_channels_last, float color_weight, float depth_weight,
+                              float normal_weight, float depth_error_max, const float *exposure, float *dL_dcolor, float *dL_ddepth,
+                              float *dL_dnormal, float *dL_dexposure, float *loss_out, void *ws, void *stream) {
+    const char *who = "rtg_loss_mapping_exposure";
+    int rc = validate_loss(who, render, depth, depth_index, gt_color, gt_depth, H, W, dL_dcolor, dL_ddepth, loss_out, ws);
+    if (rc) return rc;
+    if (!exposure || !dL_dexposure) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL exposure / dL_dexposure");
+    if (normal_weight > 0.f && (!render_normal || !gt_normal || !dL_dnormal))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": normal_weight > 0 needs render_normal, gt_normal and dL_dnormal");
+    rtg::launch_loss_mapping_exposure(render, depth, render_normal, depth_index, gt_color, gt_depth, gt_normal, render_mask, H, W,
+                                      gt_channels_last, color_weight, depth_weight, normal_weight, depth_error_max, exposure, dL_dcolor,
+                                      dL_ddepth, dL_dnormal, dL_dexposure, loss_out, ws, reinterpret_cast<cudaStream_t>(stream));
+    return check_launch(who);
+}
+
 size_t rtg_ssim_workspace_bytes(int32_t C, int32_t H, int32_t W) {
     if (C <= 0 || H <= 0 || W <= 0) return 0;
     return rtg::ssim_ws_bytes(C, H, W);
@@ -1160,6 +1185,23 @@ int rtg_ssim_loss(const float *img1, const float *img2, int32_t C, int32_t H, in
         return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_ssim_loss: bad arguments");
     rtg::launch_ssim_loss(img1, img2, C, H, W, dL_dimg1, loss_out, ws, reinterpret_cast<cudaStream_t>(stream));
     return check_launch("rtg_ssim_loss");
+}
+
+size_t rtg_ssim_exposure_workspace_bytes(int32_t C, int32_t H, int32_t W) {
+    if (C <= 0 || H <= 0 || W <= 0) return 0;
+    return rtg::ssim_exposure_ws_bytes(C, H, W);
+}
+
+int rtg_ssim_loss_exposure(const float *img1, const float *img2, int32_t C, int32_t H, int32_t W, const float *exposure,
+                           float *dL_dimg1, float *dL_dexposure, float *loss_out, void *ws, void *stream) {
+    const char *who = "rtg_ssim_loss_exposure";
+    if (!img1 || !img2 || !exposure || !loss_out || !ws) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pointer");
+    if (C <= 0 || C > 65535 || H <= 0 || W <= 0 || (H + 15) / 16 > 65535)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": bad size (C in [1, 65535], H and W >= 1, ceil(H / 16) <= 65535)");
+    if (((uintptr_t)ws) & 7) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": ws must be 8-byte aligned");
+    rtg::launch_ssim_loss_exposure(img1, img2, C, H, W, exposure, dL_dimg1, dL_dexposure, loss_out, ws,
+                                   reinterpret_cast<cudaStream_t>(stream));
+    return check_launch(who);
 }
 
 int rtg_normal_map(const float *normal, const int32_t *depth_index, int32_t H, int32_t W, float *out, void *stream) {

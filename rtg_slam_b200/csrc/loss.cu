@@ -17,6 +17,7 @@ namespace rtg {
 //                        gt_normal) (F.cosine_similarity: x.y / (max(|x|, 1e-8) * max(|y|, 1e-8))); render_normal (3,H,W),
 //                        gt_normal (H,W,3)
 //   rtg_loss_l1_exposure <false, true>   the colour residual under a frame exposure (a, b): r = e^a C + b - C^
+//   rtg_loss_mapping_exposure <true, true>  both: the mapping loss of a keyframe seen under its exposure
 // Terms, in this order: sum |r|, n_colour, sum |e|, n_depth, [normal] sum (1 - cos), n_normal, [exposure] sum sgn(r) e^a C,
 // sum sgn(r) (the last two give dL/da and dL/db). Every block of the reduce kernel writes its partial sums (no atomics); the
 // one-block final kernel adds them in a fixed order, so two calls on the same inputs give the same bits. The grad kernel's
@@ -237,6 +238,17 @@ void launch_loss_mapping(const float *render, const float *depth, const float *r
     launch_loss<true, false>(render, depth, nrm, depth_index, gt_color, gt_depth, gt_normal, mask, H, W, channels_last, color_weight,
                              depth_weight, normal_weight, depth_error_max, nullptr, dL_dcolor, dL_ddepth, dL_dnormal, nullptr, loss_out,
                              ws, s);
+}
+
+void launch_loss_mapping_exposure(const float *render, const float *depth, const float *render_normal, const int *depth_index,
+                                  const float *gt_color, const float *gt_depth, const float *gt_normal, const uint8_t *mask, int H,
+                                  int W, int channels_last, float color_weight, float depth_weight, float normal_weight,
+                                  float depth_error_max, const float *exposure, float *dL_dcolor, float *dL_ddepth,
+                                  float *dL_dnormal, float *dL_dexposure, float *loss_out, void *ws, cudaStream_t s) {
+    const float *nrm = (normal_weight > 0.f) ? render_normal : nullptr;
+    launch_loss<true, true>(render, depth, nrm, depth_index, gt_color, gt_depth, gt_normal, mask, H, W, channels_last, color_weight,
+                            depth_weight, normal_weight, depth_error_max, exposure, dL_dcolor, dL_ddepth, dL_dnormal, dL_dexposure,
+                            loss_out, ws, s);
 }
 
 // out (3,H,W) = normal[idx] where idx > -1, zeros elsewhere

@@ -28,10 +28,13 @@ struct SsimWindow {
     float g[SSIM_K];
 };
 
-// one CTA (256 threads) = one 16x16 tile of channel blockIdx.z
+// one CTA (256 threads) = one 16x16 tile of channel blockIdx.z. EXPOSURE: img1 is read as e^a img1 + b, (ea, eb) =
+// (e^a, b) (zero padding stays zero: the padded image is the exposed one).
+template <bool EXPOSURE>
 __global__ void __launch_bounds__(256) ssim_fwd_kernel(const float *__restrict__ img1, const float *__restrict__ img2, int H, int W,
                                                        const SsimWindow win, float *__restrict__ d_mu1, float *__restrict__ d_e11,
-                                                       float *__restrict__ d_e12, double *__restrict__ partial) {
+                                                       float *__restrict__ d_e12, double *__restrict__ partial,
+                                                       const float *__restrict__ exposure) {
     __shared__ float s_x[SSIM_E][SSIM_E + 1];
     __shared__ float s_y[SSIM_E][SSIM_E + 1];
     __shared__ float s_h[5][SSIM_E][SSIM_T];
@@ -39,6 +42,8 @@ __global__ void __launch_bounds__(256) ssim_fwd_kernel(const float *__restrict__
     const int tid = threadIdx.x;
     const int x0 = blockIdx.x * SSIM_T, y0 = blockIdx.y * SSIM_T;
     const size_t plane = (size_t)blockIdx.z * (size_t)H * (size_t)W;
+    float ea = 1.f, eb = 0.f;
+    if constexpr (EXPOSURE) { ea = expf(exposure[0]); eb = exposure[1]; }
 
     for (int k = tid; k < SSIM_E * SSIM_E; k += 256) {
         const int r = k / SSIM_E, q = k - r * SSIM_E;
@@ -46,7 +51,8 @@ __global__ void __launch_bounds__(256) ssim_fwd_kernel(const float *__restrict__
         float a = 0.f, b = 0.f;  // zero padding (F.conv2d(..., padding=5))
         if (gy >= 0 && gy < H && gx >= 0 && gx < W) {
             const size_t o = plane + (size_t)gy * W + gx;
-            a = img1[o];
+            if constexpr (EXPOSURE) a = fmaf(ea, img1[o], eb);
+            else a = img1[o];
             b = img2[o];
         }
         s_x[r][q] = a;
@@ -128,11 +134,15 @@ __global__ void __launch_bounds__(256) ssim_final_kernel(const double *__restric
     }
 }
 
-// dL/dimg1 for L = 1 - mean(ssim_map): scale = -1 / (C*H*W)
+// dL/dimg1 for L = 1 - mean(ssim_map): scale = -1 / (C*H*W). EXPOSURE: with x^ = e^a img1 + b the exposed image,
+// dL/dx^ is the expression below evaluated on x^, dL/dimg1 = e^a dL/dx^ (dL_dimg1 may then be NULL), and the CTA writes the
+// double partials (sum dL/dx^ e^a img1, sum dL/dx^) of dL/da and dL/db to exposure_partial[2 * CTA + {0, 1}].
+template <bool EXPOSURE>
 __global__ void __launch_bounds__(256) ssim_bwd_kernel(const float *__restrict__ img1, const float *__restrict__ img2, int H, int W,
                                                        const SsimWindow win, const float *__restrict__ d_mu1,
                                                        const float *__restrict__ d_e11, const float *__restrict__ d_e12, float scale,
-                                                       float *__restrict__ dL_dimg1) {
+                                                       float *__restrict__ dL_dimg1, const float *__restrict__ exposure,
+                                                       double *__restrict__ exposure_partial) {
     __shared__ float s_d[3][SSIM_E][SSIM_E + 1];
     __shared__ float s_h[3][SSIM_E][SSIM_T];
     const int tid = threadIdx.x;
@@ -174,10 +184,50 @@ __global__ void __launch_bounds__(256) ssim_bwd_kernel(const float *__restrict__
         c = fmaf(g, s_h[2][ty + t][tx], c);
     }
     const int gx = x0 + tx, gy = y0 + ty;
-    if (gx < W && gy < H) {
+    if constexpr (EXPOSURE) {
+        __shared__ double s_e[2][8];
+        const float ea = expf(exposure[0]), eb = exposure[1];
+        double va = 0.0, vb = 0.0;
+        if (gx < W && gy < H) {
+            const size_t o = plane + (size_t)gy * W + gx;
+            const float x = img1[o], ex = ea * x;
+            const float g = scale * (a + 2.f * fmaf(ea, x, eb) * b + img2[o] * c);
+            if (dL_dimg1) dL_dimg1[o] = ea * g;
+            va = (double)g * (double)ex;
+            vb = (double)g;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            va += __shfl_xor_sync(0xffffffffu, va, o);
+            vb += __shfl_xor_sync(0xffffffffu, vb, o);
+        }
+        if ((tid & 31) == 0) { s_e[0][tid >> 5] = va; s_e[1][tid >> 5] = vb; }
+        __syncthreads();
+        if (tid < 2) {
+            double t = 0.0;
+            for (int k = 0; k < 8; k++) t += s_e[tid][k];
+            exposure_partial[2 * (((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) + tid] = t;
+        }
+    } else if (gx < W && gy < H) {
         const size_t o = plane + (size_t)gy * W + gx;
         dL_dimg1[o] = scale * (a + 2.f * img1[o] * b + img2[o] * c);
     }
+}
+
+// dL_dexposure = (sum of the CTAs' dL/da partials, sum of their dL/db partials), added in a fixed order (bit-reproducible)
+__global__ void __launch_bounds__(256) ssim_exposure_final_kernel(const double *__restrict__ exposure_partial, int n,
+                                                                  float *__restrict__ dL_dexposure) {
+    __shared__ double s[2][256];
+    double a = 0.0, b = 0.0;
+    for (int i = threadIdx.x; i < n; i += 256) { a += exposure_partial[2 * i]; b += exposure_partial[2 * i + 1]; }
+    s[0][threadIdx.x] = a;
+    s[1][threadIdx.x] = b;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o) { s[0][threadIdx.x] += s[0][threadIdx.x + o]; s[1][threadIdx.x] += s[1][threadIdx.x + o]; }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) { dL_dexposure[0] = (float)s[0][0]; dL_dexposure[1] = (float)s[1][0]; }
 }
 
 static inline size_t ssim_tiles(int C, int H, int W) {
@@ -189,10 +239,13 @@ static inline size_t ssim_partial_bytes(int C, int H, int W) { return (ssim_tile
 // per-CTA partial sums (double) + the three derivative maps
 size_t ssim_ws_bytes(int C, int H, int W) { return ssim_partial_bytes(C, H, W) + 3 * (size_t)C * H * W * sizeof(float); }
 
-void launch_ssim_loss(const float *img1, const float *img2, int C, int H, int W, float *dL_dimg1, float *loss_out, void *ws,
-                      cudaStream_t s) {
-    ProfScope ps(K_ICP_MISC, s);
-    // gaussian(11, 1.5) of utils/loss_utils.py:40-47: fp32 values of exp(-(x-5)^2 / (2 sigma^2)), normalised in fp32
+// ssim_ws_bytes rounded up to 256 bytes (the derivative maps end on any 4-byte boundary), then the per-CTA double partials
+// of the two exposure sums
+static inline size_t ssim_exposure_partial_offset(int C, int H, int W) { return (ssim_ws_bytes(C, H, W) + 255) & ~(size_t)255; }
+size_t ssim_exposure_ws_bytes(int C, int H, int W) { return ssim_exposure_partial_offset(C, H, W) + 2 * ssim_partial_bytes(C, H, W); }
+
+// gaussian(11, 1.5) of utils/loss_utils.py:40-47: fp32 values of exp(-(x-5)^2 / (2 sigma^2)), normalised in fp32
+static SsimWindow ssim_window() {
     SsimWindow win;
     float sum = 0.f;
     for (int x = 0; x < SSIM_K; x++) {
@@ -200,15 +253,46 @@ void launch_ssim_loss(const float *img1, const float *img2, int C, int H, int W,
         sum += win.g[x];
     }
     for (int x = 0; x < SSIM_K; x++) win.g[x] /= sum;
+    return win;
+}
+
+void launch_ssim_loss(const float *img1, const float *img2, int C, int H, int W, float *dL_dimg1, float *loss_out, void *ws,
+                      cudaStream_t s) {
+    ProfScope ps(K_ICP_MISC, s);
+    const SsimWindow win = ssim_window();
     double *partial = reinterpret_cast<double *>(ws);
     const size_t n_px = (size_t)C * H * W;
     float *d_mu1 = dL_dimg1 ? reinterpret_cast<float *>(reinterpret_cast<char *>(ws) + ssim_partial_bytes(C, H, W)) : nullptr;
     float *d_e11 = dL_dimg1 ? d_mu1 + n_px : nullptr, *d_e12 = dL_dimg1 ? d_mu1 + 2 * n_px : nullptr;
     const dim3 grid((W + SSIM_T - 1) / SSIM_T, (H + SSIM_T - 1) / SSIM_T, C);
-    ssim_fwd_kernel<<<grid, 256, 0, s>>>(img1, img2, H, W, win, d_mu1, d_e11, d_e12, partial);
+    ssim_fwd_kernel<false><<<grid, 256, 0, s>>>(img1, img2, H, W, win, d_mu1, d_e11, d_e12, partial, nullptr);
     ssim_final_kernel<<<1, 256, 0, s>>>(partial, (int)ssim_tiles(C, H, W), 1.0 / (double)n_px, loss_out);
     if (dL_dimg1)
-        ssim_bwd_kernel<<<grid, 256, 0, s>>>(img1, img2, H, W, win, d_mu1, d_e11, d_e12, (float)(-1.0 / (double)n_px), dL_dimg1);
+        ssim_bwd_kernel<false><<<grid, 256, 0, s>>>(img1, img2, H, W, win, d_mu1, d_e11, d_e12, (float)(-1.0 / (double)n_px), dL_dimg1,
+                                                    nullptr, nullptr);
+}
+
+// Workspace: [value partials | derivative maps | exposure partials] (ssim_exposure_ws_bytes). The backward runs when either
+// gradient is wanted; the derivative maps are written only then.
+void launch_ssim_loss_exposure(const float *img1, const float *img2, int C, int H, int W, const float *exposure, float *dL_dimg1,
+                               float *dL_dexposure, float *loss_out, void *ws, cudaStream_t s) {
+    ProfScope ps(K_ICP_MISC, s);
+    const SsimWindow win = ssim_window();
+    double *partial = reinterpret_cast<double *>(ws);
+    const size_t n_px = (size_t)C * H * W;
+    const bool grad = dL_dimg1 || dL_dexposure;
+    char *base = reinterpret_cast<char *>(ws);
+    float *d_mu1 = grad ? reinterpret_cast<float *>(base + ssim_partial_bytes(C, H, W)) : nullptr;
+    float *d_e11 = grad ? d_mu1 + n_px : nullptr, *d_e12 = grad ? d_mu1 + 2 * n_px : nullptr;
+    double *exposure_partial = reinterpret_cast<double *>(base + ssim_exposure_partial_offset(C, H, W));
+    const int tiles = (int)ssim_tiles(C, H, W);
+    const dim3 grid((W + SSIM_T - 1) / SSIM_T, (H + SSIM_T - 1) / SSIM_T, C);
+    ssim_fwd_kernel<true><<<grid, 256, 0, s>>>(img1, img2, H, W, win, d_mu1, d_e11, d_e12, partial, exposure);
+    ssim_final_kernel<<<1, 256, 0, s>>>(partial, tiles, 1.0 / (double)n_px, loss_out);
+    if (!grad) return;
+    ssim_bwd_kernel<true><<<grid, 256, 0, s>>>(img1, img2, H, W, win, d_mu1, d_e11, d_e12, (float)(-1.0 / (double)n_px), dL_dimg1,
+                                               exposure, exposure_partial);
+    if (dL_dexposure) ssim_exposure_final_kernel<<<1, 256, 0, s>>>(exposure_partial, tiles, dL_dexposure);
 }
 
 }  // namespace rtg

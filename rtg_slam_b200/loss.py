@@ -28,6 +28,13 @@ def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def _exposure_tensor(exposure):
+    """`exposure` as the native losses read it: a (2,) CUDA float32 tensor (a, b), contiguous."""
+    if not torch.is_tensor(exposure) or not exposure.is_cuda or exposure.dtype != torch.float32 or exposure.shape != (2,):
+        raise TypeError("exposure must be a (2,) CUDA float32 tensor")
+    return exposure.contiguous()
+
+
 def frame_targets(gt_color, gt_depth, render_mask, H, W):
     """A measured H x W frame as the native losses and pose steps read it: (gt_color, gt_depth, mask, channels_last).
     gt_color (H,W,3) (channels_last = 1) or (3,H,W) (0) and gt_depth with H*W elements, both CUDA float32, come back
@@ -54,7 +61,8 @@ def frame_targets(gt_color, gt_depth, render_mask, H, W):
 
 class _FusedLoss(torch.autograd.Function):
     """The frame loss and its gradients from one native call: rtg_loss_mapping if `mapping` (with the normal term when
-    `normal` is given), else rtg_loss_l1_exposure if `exposure` is given, else rtg_loss_l1. Returns (loss, parts)."""
+    `normal` is given; rtg_loss_mapping_exposure if `exposure` is given too), else rtg_loss_l1_exposure if `exposure` is
+    given, else rtg_loss_l1. Returns (loss, parts)."""
 
     @staticmethod
     def forward(ctx, render, depth, normal, exposure, depth_index, gt_color, gt_depth, gt_normal, render_mask, weights, mapping):
@@ -73,23 +81,27 @@ class _FusedLoss(torch.autograd.Function):
         out = torch.empty(8 if mapping else 4, dtype=torch.float32, device=dev)
         frame = (_p(depth_index), _p(gt_color), _p(gt_depth))
         stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        if exposure is not None:
+            exposure = _exposure_tensor(exposure)
+            g_exposure = torch.empty(2, dtype=torch.float32, device=dev)
         if mapping:
             if normal is not None:
                 normal, gt_normal = normal.contiguous(), gt_normal.contiguous()
                 if normal.shape != (3, H, W) or gt_normal.shape != (H, W, 3):
                     raise ValueError("normal must be (3,H,W) and gt_normal (H,W,3)")
                 g_normal = torch.empty_like(render)
-            check(L.rtg_loss_mapping(_p(render), _p(depth), _p(normal), *frame, _p(gt_normal), _p(mask), H, W, channels_last,
-                                     color_weight, depth_weight, normal_weight, depth_error_max, _p(g_color), _p(g_depth),
-                                     _p(g_normal), _p(out), _p(_ws(dev)), stream), "rtg_loss_mapping")
+            head = (_p(render), _p(depth), _p(normal), *frame, _p(gt_normal), _p(mask), H, W, channels_last, color_weight, depth_weight,
+                    normal_weight, depth_error_max)
+            if exposure is None:
+                check(L.rtg_loss_mapping(*head, _p(g_color), _p(g_depth), _p(g_normal), _p(out), _p(_ws(dev)), stream),
+                      "rtg_loss_mapping")
+            else:
+                check(L.rtg_loss_mapping_exposure(*head, _p(exposure), _p(g_color), _p(g_depth), _p(g_normal), _p(g_exposure), _p(out),
+                                                  _p(_ws(dev)), stream), "rtg_loss_mapping_exposure")
         elif exposure is None:
             check(L.rtg_loss_l1(_p(render), _p(depth), *frame, _p(mask), H, W, channels_last, color_weight, depth_weight,
                                 depth_error_max, _p(g_color), _p(g_depth), _p(out), _p(_ws(dev)), stream), "rtg_loss_l1")
         else:
-            if not exposure.is_cuda or exposure.dtype != torch.float32 or exposure.shape != (2,):
-                raise TypeError("exposure must be a (2,) CUDA float32 tensor")
-            exposure = exposure.contiguous()
-            g_exposure = torch.empty(2, dtype=torch.float32, device=dev)
             check(L.rtg_loss_l1_exposure(_p(render), _p(depth), *frame, _p(mask), H, W, channels_last, color_weight, depth_weight,
                                          depth_error_max, _p(exposure), _p(g_color), _p(g_depth), _p(g_exposure), _p(out),
                                          _p(_ws(dev)), stream), "rtg_loss_l1_exposure")
@@ -120,10 +132,11 @@ _SSIM_WS = {}
 class _FusedSsim(torch.autograd.Function):
     """1 - ssim(img1, img2) of utils/loss_utils.py:40-100 (11x11 Gaussian window, sigma 1.5, zero padding, mean) and its
     gradient w.r.t. img1 from three kernels (rtg_ssim_loss) instead of five grouped convolutions + ~15 elementwise kernels
-    and their autograd twins. img2 (the measured frame) gets no gradient."""
+    and their autograd twins. img2 (the measured frame) gets no gradient. With `exposure` (a, b) it is
+    1 - ssim(e^a img1 + b, img2) (rtg_ssim_loss_exposure), differentiable w.r.t. img1 and the exposure."""
 
     @staticmethod
-    def forward(ctx, img1, img2):
+    def forward(ctx, img1, img2, exposure):
         L = _lib.lib()
         if img1.dim() != 3 or img1.shape != img2.shape:
             raise ValueError("ssim_loss: img1 and img2 must both be (C,H,W)")
@@ -133,7 +146,10 @@ class _FusedSsim(torch.autograd.Function):
         dev = img1.device
         Cn, H, W = img1.shape
         a, b = img1.contiguous(), img2.contiguous()
-        need = int(L.rtg_ssim_workspace_bytes(Cn, H, W))
+        if exposure is not None:
+            exposure = _exposure_tensor(exposure)
+        ws_bytes = L.rtg_ssim_workspace_bytes if exposure is None else L.rtg_ssim_exposure_workspace_bytes
+        need = int(ws_bytes(Cn, H, W))
         idx = dev.index if dev.index is not None else torch.cuda.current_device()
         ws = _SSIM_WS.get(idx)
         if ws is None or ws.numel() < need:
@@ -143,22 +159,29 @@ class _FusedSsim(torch.autograd.Function):
         want_grad = ctx.needs_input_grad[0]
         g = torch.empty_like(a) if want_grad else None
         out = torch.empty(2, dtype=torch.float32, device=dev)
-        check(L.rtg_ssim_loss(_p(a), _p(b), Cn, H, W, _p(g), _p(out), _p(ws), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-              "rtg_ssim_loss")
-        if want_grad:
-            ctx.save_for_backward(g)
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        g_exposure = None
+        if exposure is None:
+            check(L.rtg_ssim_loss(_p(a), _p(b), Cn, H, W, _p(g), _p(out), _p(ws), stream), "rtg_ssim_loss")
+        else:
+            g_exposure = torch.empty(2, dtype=torch.float32, device=dev) if ctx.needs_input_grad[2] else None
+            check(L.rtg_ssim_loss_exposure(_p(a), _p(b), Cn, H, W, _p(exposure), _p(g), _p(g_exposure), _p(out), _p(ws), stream),
+                  "rtg_ssim_loss_exposure")
+        ctx.save_for_backward(g, g_exposure)
         return out[0]
 
     @staticmethod
     def backward(ctx, grad_loss):
-        (g,) = ctx.saved_tensors
-        return g * grad_loss, None
+        g, g_exposure = ctx.saved_tensors
+        return (None if g is None else g * grad_loss), None, (None if g_exposure is None else g_exposure * grad_loss)
 
 
-def ssim_loss(img1, img2):
+def ssim_loss(img1, img2, exposure=None):
     """`1 - ssim(img1, img2)` as Mapping.loss_update evaluates it (SLAM/multiprocess/mapper.py:411-415, utils/loss_utils.py:50-100);
-    img1, img2: (C,H,W) CUDA float32. Differentiable w.r.t. img1."""
-    return _FusedSsim.apply(img1, img2)
+    img1, img2: (C,H,W) CUDA float32. Differentiable w.r.t. img1.
+    `exposure`: None, or a (2,) CUDA float32 tensor (a, b): the term becomes 1 - ssim(e^a img1 + b, img2)
+    (rtg_ssim_loss_exposure), differentiable w.r.t. img1 and `exposure`."""
+    return _FusedSsim.apply(img1, img2, exposure)
 
 
 def _ssim_term(img1, img2, window_size=11):
@@ -183,24 +206,28 @@ def _ssim_term(img1, img2, window_size=11):
 
 
 def mapping_loss(render_output, image_input, render_mask=None, color_weight=0.8, depth_weight=1.0, normal_weight=0.0, ssim_weight=0.2,
-                 depth_error_max=0.1):
+                 depth_error_max=0.1, exposure=None):
     """The image-space part of `Mapping.loss_update` (SLAM/multiprocess/mapper.py:402-451): colour L1 on the render mask,
     depth L1 on the valid mask, cosine normal loss, and -- only without a render mask, as in the reference -- the SSIM
     term. `render_output`: dict of Renderer.render; `image_input`: dict with "color_map" (H,W,3), "depth_map" (H,W[,1]),
     "normal_map" (H,W,3). Colour, depth and normal terms and their gradients come from three fused kernels, the SSIM term
     (which the shipped flows never reach: both call sites pass a render mask) from three more (`ssim_loss`).
     Returns (total_loss, parts): parts is a device tensor {total, colour, depth, n_depth, normal, n_normal, ssim, 0} --
-    read it back once with `report_losses` instead of six `.item()` calls (mapper.py:459-466)."""
+    read it back once with `report_losses` instead of six `.item()` calls (mapper.py:459-466).
+    `exposure`: None, or a (2,) CUDA float32 tensor (a, b), e.g. `keyframes.KeyframeTable.exposure(k)`: the colour L1 and the
+    SSIM term are taken on e^a render + b (rtg_loss_mapping_exposure, `ssim_loss(..., exposure=)`), so that a keyframe seen
+    brighter or darker than the map is fitted without baking its brightness into the map; autograd sums the two terms'
+    exposure gradients. The depth and normal terms do not see it."""
     nrm, gtn = render_output.get("normal"), image_input.get("normal_map")
     if not (normal_weight > 0 and nrm is not None and gtn is not None):
         nrm, gtn, normal_weight = None, None, 0.0
-    loss, parts = _FusedLoss.apply(render_output["render"], render_output["depth"], nrm, None, render_output["depth_index_map"],
+    loss, parts = _FusedLoss.apply(render_output["render"], render_output["depth"], nrm, exposure, render_output["depth_index_map"],
                                    image_input["color_map"], image_input["depth_map"], gtn, render_mask,
                                    (color_weight, depth_weight, normal_weight, depth_error_max), True)
     if render_mask is None and ssim_weight > 0:
         gt = image_input["color_map"]
         gt = gt.permute(2, 0, 1) if gt.shape[-1] == 3 and gt.dim() == 3 and gt.shape[0] != 3 else gt
-        ssim_l = ssim_loss(render_output["render"], gt)
+        ssim_l = ssim_loss(render_output["render"], gt, exposure)
         loss = loss + ssim_weight * ssim_l
         parts = parts.clone()
         parts[6] = ssim_l.detach()

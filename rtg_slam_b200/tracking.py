@@ -173,6 +173,16 @@ def downsample_frame(gt_color, gt_depth, s, render_mask=None, tile_mask=None):
     return color, depth, mask_out, tmask_out
 
 
+def camera_tensors(pose, projection):
+    """The three camera tensors the rasterizer reads, as rtg_pose_adam_step writes them: viewmatrix = W2C^T, projmatrix =
+    viewmatrix @ projection and campos = -R^T t, float32 and contiguous, from the double W2C `pose` (4, 4) and the float32
+    `projection` (4, 4)."""
+    view = pose.t().float().contiguous()
+    proj = (pose.t() @ projection.double()).float().contiguous()
+    campos = (-(pose[:3, :3].t() @ pose[:3, 3])).float().contiguous()
+    return view, proj, campos
+
+
 class PoseRefiner:
     """Refines a world-to-camera pose against a frozen Gaussian map. `args` is the bag `render.Renderer` takes."""
 
@@ -197,9 +207,7 @@ class PoseRefiner:
         vm0 = camera.world_view_transform.detach().to(device=dev, dtype=torch.float64)
         pose = vm0.t().contiguous()                                   # W2C, row-major, double
         projection = camera.projection_matrix.detach().to(device=dev, dtype=torch.float32).contiguous()
-        view = pose.t().float().contiguous().requires_grad_(requires_grad)
-        proj = (pose.t() @ projection.double()).float().contiguous().requires_grad_(requires_grad)
-        campos = (-(pose[:3, :3].t() @ pose[:3, 3])).float().contiguous().requires_grad_(requires_grad)
+        view, proj, campos = (t.requires_grad_(requires_grad) for t in camera_tensors(pose, projection))
         rs = self._settings(camera, dev, view, proj, campos)
         g = {k: gaussian_data[k].detach() for k in ("xyz", "opacity", "shs", "scales", "rotations")}
         return dev, pose, projection, view, proj, campos, rs, g

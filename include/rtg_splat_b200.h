@@ -827,6 +827,49 @@ typedef struct RtgMapTransform {
 size_t rtg_map_transform_workspace_bytes(int32_t K);
 int rtg_map_transform(const RtgMapTransform *xf, void *ws, void *stream);
 
+/* ---- a surface from the map: TSDF fusion and marching tetrahedra (no reference counterpart) ------------------------
+ * RtgTsdfVolume describes a dense voxel grid owned by the caller: voxel (i,j,k) has its centre at origin + voxel_size *
+ * (i,j,k); tsdf, weight and color are structure-of-arrays, x fastest (linear index i + nx*(j + ny*k)), float32, with
+ * color as three planes of nx*ny*nz floats (R, G, B) or NULL. A fresh volume holds tsdf = 1, weight = 0, color = 0.
+ * nx, ny, nz >= 1 and nx*ny*nz < 2^31; voxel_size > 0; trunc > 0 in map units.
+ *
+ * rtg_tsdf_integrate folds one depth frame into the volume. For every voxel, with p_c = R p + t of the W2C `w2c`:
+ *   skip if z <= 0; (u, v) = (fx x/z + cx, fy y/z + cy), pixel (rint(u), rint(v)) with rounding half to even, skip if
+ *   outside the image; d = depth[pixel], skip if d <= 0 (0 = no reading / no hit); sdf = d - z, skip if sdf < -trunc;
+ *   f = min(1, sdf / trunc); tsdf <- (tsdf w + f)/(w + 1), color <- (color w + c_pixel)/(w + 1), w <- w + 1.
+ * depth (H,W) float32; color (3,H,W), or (H,W,3) with color_channels_last = 1, given exactly when the volume has color;
+ * w2c: 16 row-major doubles (w2c_is_double = 1) or floats (0) in device memory, read on the device. Arithmetic is float64.
+ * A voxel is written only when it is updated; there are no atomics, so equal call sequences give equal bits, and no host
+ * synchronisation.
+ *
+ * Extraction (marching tetrahedra on the Kuhn decomposition: cell (i,j,k), i < nx-1 etc., splits into six tetrahedra,
+ * one per axis permutation p in lexicographic order, c -> c+e_p0 -> c+e_p0+e_p1 -> c+(1,1,1)). Voxel a owns the edges to
+ * a + (1,0,0), (0,1,0), (0,0,1), (1,1,0), (0,1,1), (1,0,1), (1,1,1) (slots 0..6). An edge (a, b) carries a vertex when both
+ * weights are > 0 and exactly one of its tsdf values is < 0; it lies at a + tau (b - a), tau = f_a / (f_a - f_b), in world
+ * units, with the colour interpolated with the same tau. A tetrahedron whose four weights are > 0 emits one triangle
+ * with one or three negative corners and two with two; winding is right-handed, the normal pointing from negative to
+ * positive tsdf. Vertices are ordered by (owning voxel, slot), triangles by (cell, tetrahedron, triangle 0..1).
+ *   rtg_tsdf_extract_count: one counting pass and two exclusive scans; writes counts[0] = vertices, counts[1] =
+ *     triangles (device uint32[2]) and keeps the offsets in ws (rtg_tsdf_extract_workspace_bytes(nx, ny, nz) bytes).
+ *   rtg_tsdf_extract_emit: with the same ws and an unchanged volume, writes vertices (V,3) float32, vertex_colors (V,3)
+ *     float32 (may be NULL; ignored without volume color) and faces (F,3) int32. Writes stay inside the counted ranges.
+ * Extraction needs 12 * nx*ny*nz < 2^32 (at most 12 triangles per cell, uint32 offsets).
+ * Every entry point validates on the host before any CUDA call: a NULL descriptor or required pointer, non-positive sizes,
+ * voxel_size or trunc, and a voxel count at or above the limit are rejected. */
+typedef struct RtgTsdfVolume {
+    int32_t nx, ny, nz;
+    float voxel_size, trunc;
+    float origin[3];
+    float *tsdf, *weight, *color;
+} RtgTsdfVolume;
+int rtg_tsdf_integrate(const RtgTsdfVolume *vol, const float *depth, const float *color, int32_t H, int32_t W,
+                       int32_t color_channels_last, float fx, float fy, float cx, float cy, const void *w2c, int32_t w2c_is_double,
+                       void *stream);
+size_t rtg_tsdf_extract_workspace_bytes(int32_t nx, int32_t ny, int32_t nz);
+int rtg_tsdf_extract_count(const RtgTsdfVolume *vol, void *ws, uint32_t *counts, void *stream);
+int rtg_tsdf_extract_emit(const RtgTsdfVolume *vol, const void *ws, float *vertices, float *vertex_colors, int32_t *faces,
+                          void *stream);
+
 /* ---- measurement hook (no reference counterpart) ---------------------------------------------
  * When enabled, every kernel launch of this library is bracketed by CUDA events on its launching stream.
  * rtg_profile_read synchronises the device and returns, per kernel id, the summed duration (ms) and the number

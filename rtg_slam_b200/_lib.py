@@ -100,6 +100,13 @@ class RtgMapTransform(C.Structure):
                                              "n_skipped")])
 
 
+class RtgTsdfVolume(C.Structure):
+    """include/rtg_splat_b200.h: RtgTsdfVolume (field order is the ABI)."""
+    _fields_ = ([(n, C.c_int32) for n in ("nx", "ny", "nz")] + [("voxel_size", C.c_float), ("trunc", C.c_float),
+                                                               ("origin", C.c_float * 3)]
+                + [(n, C.c_void_p) for n in ("tsdf", "weight", "color")])
+
+
 class RtgIcpLevel(C.Structure):
     _fields_ = [("vertex0", C.c_void_p), ("normal0", C.c_void_p), ("vertex1", C.c_void_p), ("normal1", C.c_void_p),
                 ("H", C.c_int32), ("W", C.c_int32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
@@ -200,6 +207,11 @@ SIGNATURES = {
     "rtg_knn": (C.c_int, [_VP, _I64, _VP, _I64, _I32, _I32, _VP, _VP, _VP, _VP, _VP]),
     "rtg_map_transform_workspace_bytes": (C.c_size_t, [_I32]),
     "rtg_map_transform": (C.c_int, [C.POINTER(RtgMapTransform), _VP, _VP]),
+    # vol, depth, color, H, W, color_channels_last, fx, fy, cx, cy, w2c, w2c_is_double, stream
+    "rtg_tsdf_integrate": (C.c_int, [C.POINTER(RtgTsdfVolume), _VP, _VP, _I32, _I32, _I32, _F, _F, _F, _F, _VP, _I32, _VP]),
+    "rtg_tsdf_extract_workspace_bytes": (C.c_size_t, [_I32, _I32, _I32]),
+    "rtg_tsdf_extract_count": (C.c_int, [C.POINTER(RtgTsdfVolume), _VP, _VP, _VP]),
+    "rtg_tsdf_extract_emit": (C.c_int, [C.POINTER(RtgTsdfVolume), _VP, _VP, _VP, _VP, _VP]),
     "rtg_profile_enable": (C.c_int, [_I32]),
     "rtg_profile_kernel_count": (C.c_int, []),
     "rtg_profile_kernel_name": (C.c_char_p, [_I32]),

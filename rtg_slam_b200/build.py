@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librtg_splat_b200.so")
-SOURCES = ["capi.cu", "preprocess.cu", "binning.cu", "render.cu", "adam.cu", "icp.cu", "loss.cu", "ssim.cu", "mapstats.cu", "frameprep.cu", "mapsurgery.cu", "mapstep.cu", "maptransform.cu"]
+SOURCES = ["capi.cu", "preprocess.cu", "binning.cu", "render.cu", "adam.cu", "icp.cu", "loss.cu", "ssim.cu", "mapstats.cu", "frameprep.cu", "mapsurgery.cu", "mapstep.cu", "maptransform.cu", "tsdf.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
     *ARCH, "-lineinfo", "-O3", "-std=c++17",

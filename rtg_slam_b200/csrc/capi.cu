@@ -97,7 +97,8 @@ void prof_end(int id, cudaStream_t s) {
     g_prof_recs.push_back({id, t_open[id], e});
 }
 static const char *kKernelNames[K_COUNT] = {"preprocess_fwd", "tile_scan", "scatter", "tile_sort", "render_fwd", "render_bwd",
-                                            "preprocess_bwd", "adam", "icp_build_level", "icp_iter", "image_glue", "bwd_zero"};
+                                            "preprocess_bwd", "adam", "icp_build_level", "icp_iter", "image_glue", "bwd_zero",
+                                            "tsdf_integrate", "tsdf_extract"};
 }  // namespace rtg
 
 static thread_local std::string g_err;
@@ -1338,6 +1339,64 @@ int rtg_map_transform(const RtgMapTransform *xf, void *ws, void *stream) {
     if (reinterpret_cast<uintptr_t>(ws) & 15) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_map_transform: ws must be 16-byte aligned");
     rtg::launch_map_transform(*xf, ws, s);
     return check_launch("rtg_map_transform");
+}
+
+// the voxel count, or -1 when the sizes are not positive or nx*ny*nz >= limit
+static int64_t tsdf_voxels(int32_t nx, int32_t ny, int32_t nz, int64_t limit) {
+    if (nx <= 0 || ny <= 0 || nz <= 0) return -1;
+    if ((int64_t)nx * ny >= limit) return -1;  // then nx*ny < 2^32 and the full product fits int64
+    const int64_t n = (int64_t)nx * ny * nz;
+    return n >= limit ? -1 : n;
+}
+
+static int validate_tsdf_volume(const char *who, const RtgTsdfVolume *v, int64_t limit) {
+    if (!v) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": vol is NULL");
+    if (tsdf_voxels(v->nx, v->ny, v->nz, limit) < 0)
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": bad dims (each >= 1, nx*ny*nz below the limit)");
+    if (!(v->voxel_size > 0.f) || !(v->trunc > 0.f) || !std::isfinite(v->voxel_size) || !std::isfinite(v->trunc))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": voxel_size and trunc must be finite and > 0");
+    if (!std::isfinite(v->origin[0]) || !std::isfinite(v->origin[1]) || !std::isfinite(v->origin[2]))
+        return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": origin must be finite");
+    if (!v->tsdf || !v->weight) return fail(RTG_ERR_INVALID_ARGUMENT, std::string(who) + ": NULL pointer (tsdf or weight)");
+    return RTG_OK;
+}
+
+static const int64_t kTsdfMaxVoxels = 0x80000000LL;            // 2^31
+static const int64_t kTsdfMaxExtractVoxels = 0x100000000LL / 12;  // 12 triangles per cell must fit uint32 offsets
+
+int rtg_tsdf_integrate(const RtgTsdfVolume *vol, const float *depth, const float *color, int32_t H, int32_t W,
+                       int32_t color_channels_last, float fx, float fy, float cx, float cy, const void *w2c, int32_t w2c_is_double,
+                       void *stream) {
+    if (int rc = validate_tsdf_volume("rtg_tsdf_integrate", vol, kTsdfMaxVoxels)) return rc;
+    if (H <= 0 || W <= 0) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_integrate: bad image size (H, W >= 1)");
+    if (!depth || !w2c) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_integrate: NULL pointer (depth or w2c)");
+    if ((vol->color == nullptr) != (color == nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_integrate: color must be given exactly when the volume has color");
+    if (!std::isfinite(fx) || !std::isfinite(fy) || !std::isfinite(cx) || !std::isfinite(cy) || fx == 0.f || fy == 0.f)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_integrate: intrinsics must be finite with fx, fy != 0");
+    rtg::launch_tsdf_integrate(*vol, depth, color, H, W, color_channels_last != 0, fx, fy, cx, cy, w2c, w2c_is_double != 0,
+                               reinterpret_cast<cudaStream_t>(stream));
+    return check_launch("rtg_tsdf_integrate");
+}
+
+size_t rtg_tsdf_extract_workspace_bytes(int32_t nx, int32_t ny, int32_t nz) {
+    const int64_t n = tsdf_voxels(nx, ny, nz, kTsdfMaxExtractVoxels);
+    return n < 0 ? 0 : rtg::tsdf_extract_ws_bytes(n);
+}
+
+int rtg_tsdf_extract_count(const RtgTsdfVolume *vol, void *ws, uint32_t *counts, void *stream) {
+    if (int rc = validate_tsdf_volume("rtg_tsdf_extract_count", vol, kTsdfMaxExtractVoxels)) return rc;
+    if (!ws || !counts) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_extract_count: NULL pointer (ws or counts)");
+    rtg::launch_tsdf_extract_count(*vol, ws, counts, reinterpret_cast<cudaStream_t>(stream));
+    return check_launch("rtg_tsdf_extract_count");
+}
+
+int rtg_tsdf_extract_emit(const RtgTsdfVolume *vol, const void *ws, float *vertices, float *vertex_colors, int32_t *faces,
+                          void *stream) {
+    if (int rc = validate_tsdf_volume("rtg_tsdf_extract_emit", vol, kTsdfMaxExtractVoxels)) return rc;
+    if (!ws || !vertices || !faces) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_extract_emit: NULL pointer (ws, vertices or faces)");
+    rtg::launch_tsdf_extract_emit(*vol, ws, vertices, vertex_colors, faces, reinterpret_cast<cudaStream_t>(stream));
+    return check_launch("rtg_tsdf_extract_emit");
 }
 
 int rtg_profile_enable(int32_t on) {

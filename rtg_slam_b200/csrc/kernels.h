@@ -3,6 +3,7 @@
 #include "common.cuh"
 
 struct RtgMapTransform;
+struct RtgTsdfVolume;
 
 namespace rtg {
 
@@ -138,6 +139,11 @@ void launch_icp_intensity_pyramid(const IcpIntensity &prm, cudaStream_t s);
 size_t soa_compact_ws_bytes(int64_t P);
 void launch_soa_compact(const uint8_t *mask, int invert, int64_t P, int n_arrays, const void *const *in, void *const *out,
                         const int32_t *words_per_row, uint32_t *n_kept, uint32_t *n_kept_host, void *ws, cudaStream_t s);
+// out[i] = sum of in[0..i) (out may be in: each element is read before it is overwritten); sums: scratch of
+// exclusive_scan_sums_words(n) words; total (device) / total_host (mapped) may be NULL
+size_t exclusive_scan_sums_words(uint32_t n);
+void exclusive_scan_u32(const uint32_t *in, uint32_t n, uint32_t *out, uint32_t *sums, uint32_t *total, uint32_t *total_host,
+                        cudaStream_t s);
 size_t knn_ws_bytes(int64_t n_ref);
 int launch_knn(const float *query, int64_t n_query, const float *ref, int64_t n_ref, int K, int skip_self, float *out_d2, int32_t *out_idx,
                float *out_mean, void *ws, cudaStream_t s);
@@ -145,6 +151,14 @@ int launch_knn(const float *query, int64_t n_query, const float *ref, int64_t n_
 // maptransform.cu
 size_t map_transform_ws_bytes(int64_t K);
 void launch_map_transform(const RtgMapTransform &m, void *ws, cudaStream_t s);
+
+// tsdf.cu
+void launch_tsdf_integrate(const RtgTsdfVolume &v, const float *depth, const float *color, int H, int W, int channels_last, float fx,
+                           float fy, float cx, float cy, const void *w2c, bool w2c_double, cudaStream_t s);
+size_t tsdf_extract_ws_bytes(int64_t n);
+void launch_tsdf_extract_count(const RtgTsdfVolume &v, void *ws, uint32_t *counts, cudaStream_t s);
+void launch_tsdf_extract_emit(const RtgTsdfVolume &v, const void *ws, float *vertices, float *vertex_colors, int32_t *faces,
+                              cudaStream_t s);
 
 // adam.cu and the per-level icp.cu entry points are declared in their own sections of capi.cu
 }  // namespace rtg

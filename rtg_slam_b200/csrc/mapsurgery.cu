@@ -89,9 +89,11 @@ __global__ void __launch_bounds__(SCAN_BLOCK) scan_apply_kernel(const uint32_t *
     if (i < n) out[i] = sums[blockIdx.x] + ex;
 }
 
+size_t exclusive_scan_sums_words(uint32_t n) { return (n + SCAN_BLOCK - 1) / SCAN_BLOCK; }
+
 // out[i] = sum of in[0..i); sums: scratch of ceil(n / 1024) words; total (device) / total_host (mapped) may be NULL
-static void exclusive_scan_u32(const uint32_t *in, uint32_t n, uint32_t *out, uint32_t *sums, uint32_t *total, uint32_t *total_host,
-                               cudaStream_t s) {
+void exclusive_scan_u32(const uint32_t *in, uint32_t n, uint32_t *out, uint32_t *sums, uint32_t *total, uint32_t *total_host,
+                        cudaStream_t s) {
     const uint32_t nb = (n + SCAN_BLOCK - 1) / SCAN_BLOCK;
     scan_block_sums_kernel<<<nb, SCAN_BLOCK, 0, s>>>(in, n, sums);
     scan_sums_kernel<<<1, SCAN_BLOCK, 0, s>>>(sums, nb, total, total_host);

@@ -865,6 +865,24 @@ typedef struct RtgTsdfVolume {
 int rtg_tsdf_integrate(const RtgTsdfVolume *vol, const float *depth, const float *color, int32_t H, int32_t W,
                        int32_t color_channels_last, float fx, float fy, float cx, float cy, const void *w2c, int32_t w2c_is_double,
                        void *stream);
+/* rtg_tsdf_raycast renders the surface extraction emits, seen from the W2C `w2c` (16 row-major doubles or floats in
+ * device memory, read on the device; arithmetic in float64, outputs rounded once to float32). Pixel (u, v) has the ray
+ * o + t d, o = -R^T t_w2c, d = R^T ((u - cx)/fx, (v - cy)/fy, 1), so t is camera z; it starts at t > 0 and ends where it
+ * leaves the cell region [origin, origin + voxel_size (n - 1)]. The field is the piecewise-linear interpolant on the Kuhn
+ * tetrahedra of extraction (not trilinear): in cell c with local u in [0,1]^3, the tetrahedron of the permutation p that
+ * orders u decreasingly has the weights 1 - u_p1, u_p1 - u_p2, u_p2 - u_p3, u_p3 on c, c+e_p1, c+e_p1+e_p2, c+(1,1,1);
+ * only tetrahedra whose four weights are > 0 take part. Cells are walked in ray order, each cut at the planes u_a = u_b
+ * into pieces of one tetrahedron; along a piece the field is linear and its zero is t* = t_s + (t_e - t_s) f_s/(f_s - f_e).
+ * The first piece whose field changes sign (sign test f < 0) decides: from >= 0 to < 0 it is a hit, with depth t*,
+ * normal the tetrahedron's unit gradient (world space, towards free space: the face normal of the mesh triangle) and
+ * colour interpolated with the tetrahedron's weights (the mesh's vertex colours interpolated over the triangle); from < 0
+ * to >= 0 it is a back face and the ray ends without a hit. Pixels without a hit get depth 0, normal 0 and colour 0.
+ * depth (H,W) float32; normal (3,H,W) float32; color (3,H,W) float32, given exactly when the volume has color.
+ * One thread per pixel; no atomics (repeats give equal bits) and no host synchronisation. Validated like
+ * rtg_tsdf_integrate: volume (nx*ny*nz < 2^31), H, W >= 1, NULL pointers, colour against the volume, finite intrinsics
+ * with fx, fy != 0. */
+int rtg_tsdf_raycast(const RtgTsdfVolume *vol, const void *w2c, int32_t w2c_is_double, int32_t H, int32_t W, float fx, float fy,
+                     float cx, float cy, float *depth, float *normal, float *color, void *stream);
 size_t rtg_tsdf_extract_workspace_bytes(int32_t nx, int32_t ny, int32_t nz);
 int rtg_tsdf_extract_count(const RtgTsdfVolume *vol, void *ws, uint32_t *counts, void *stream);
 int rtg_tsdf_extract_emit(const RtgTsdfVolume *vol, const void *ws, float *vertices, float *vertex_colors, int32_t *faces,

@@ -209,6 +209,8 @@ SIGNATURES = {
     "rtg_map_transform": (C.c_int, [C.POINTER(RtgMapTransform), _VP, _VP]),
     # vol, depth, color, H, W, color_channels_last, fx, fy, cx, cy, w2c, w2c_is_double, stream
     "rtg_tsdf_integrate": (C.c_int, [C.POINTER(RtgTsdfVolume), _VP, _VP, _I32, _I32, _I32, _F, _F, _F, _F, _VP, _I32, _VP]),
+    # vol, w2c, w2c_is_double, H, W, fx, fy, cx, cy, depth, normal, color, stream
+    "rtg_tsdf_raycast": (C.c_int, [C.POINTER(RtgTsdfVolume), _VP, _I32, _I32, _I32, _F, _F, _F, _F, _VP, _VP, _VP, _VP]),
     "rtg_tsdf_extract_workspace_bytes": (C.c_size_t, [_I32, _I32, _I32]),
     "rtg_tsdf_extract_count": (C.c_int, [C.POINTER(RtgTsdfVolume), _VP, _VP, _VP]),
     "rtg_tsdf_extract_emit": (C.c_int, [C.POINTER(RtgTsdfVolume), _VP, _VP, _VP, _VP, _VP]),

@@ -98,7 +98,7 @@ void prof_end(int id, cudaStream_t s) {
 }
 static const char *kKernelNames[K_COUNT] = {"preprocess_fwd", "tile_scan", "scatter", "tile_sort", "render_fwd", "render_bwd",
                                             "preprocess_bwd", "adam", "icp_build_level", "icp_iter", "image_glue", "bwd_zero",
-                                            "tsdf_integrate", "tsdf_extract"};
+                                            "tsdf_integrate", "tsdf_extract", "tsdf_raycast"};
 }  // namespace rtg
 
 static thread_local std::string g_err;
@@ -1377,6 +1377,20 @@ int rtg_tsdf_integrate(const RtgTsdfVolume *vol, const float *depth, const float
     rtg::launch_tsdf_integrate(*vol, depth, color, H, W, color_channels_last != 0, fx, fy, cx, cy, w2c, w2c_is_double != 0,
                                reinterpret_cast<cudaStream_t>(stream));
     return check_launch("rtg_tsdf_integrate");
+}
+
+int rtg_tsdf_raycast(const RtgTsdfVolume *vol, const void *w2c, int32_t w2c_is_double, int32_t H, int32_t W, float fx, float fy,
+                     float cx, float cy, float *depth, float *normal, float *color, void *stream) {
+    if (int rc = validate_tsdf_volume("rtg_tsdf_raycast", vol, kTsdfMaxVoxels)) return rc;
+    if (H <= 0 || W <= 0) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_raycast: bad image size (H, W >= 1)");
+    if (!w2c || !depth || !normal) return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_raycast: NULL pointer (w2c, depth or normal)");
+    if ((vol->color == nullptr) != (color == nullptr))
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_raycast: color must be given exactly when the volume has color");
+    if (!std::isfinite(fx) || !std::isfinite(fy) || !std::isfinite(cx) || !std::isfinite(cy) || fx == 0.f || fy == 0.f)
+        return fail(RTG_ERR_INVALID_ARGUMENT, "rtg_tsdf_raycast: intrinsics must be finite with fx, fy != 0");
+    rtg::launch_tsdf_raycast(*vol, w2c, w2c_is_double != 0, H, W, fx, fy, cx, cy, depth, normal, color,
+                             reinterpret_cast<cudaStream_t>(stream));
+    return check_launch("rtg_tsdf_raycast");
 }
 
 size_t rtg_tsdf_extract_workspace_bytes(int32_t nx, int32_t ny, int32_t nz) {

@@ -155,6 +155,8 @@ void launch_map_transform(const RtgMapTransform &m, void *ws, cudaStream_t s);
 // tsdf.cu
 void launch_tsdf_integrate(const RtgTsdfVolume &v, const float *depth, const float *color, int H, int W, int channels_last, float fx,
                            float fy, float cx, float cy, const void *w2c, bool w2c_double, cudaStream_t s);
+void launch_tsdf_raycast(const RtgTsdfVolume &v, const void *w2c, bool w2c_double, int H, int W, float fx, float fy, float cx,
+                         float cy, float *depth, float *normal, float *color, cudaStream_t s);
 size_t tsdf_extract_ws_bytes(int64_t n);
 void launch_tsdf_extract_count(const RtgTsdfVolume &v, void *ws, uint32_t *counts, cudaStream_t s);
 void launch_tsdf_extract_emit(const RtgTsdfVolume &v, const void *ws, float *vertices, float *vertex_colors, int32_t *faces,

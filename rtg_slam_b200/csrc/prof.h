@@ -7,7 +7,7 @@ namespace rtg {
 
 enum KernelId {
     K_PREPROCESS_FWD = 0, K_TILE_SCAN, K_SCATTER, K_TILE_SORT, K_RENDER_FWD, K_RENDER_BWD, K_PREPROCESS_BWD, K_ADAM,
-    K_ICP_BUILD, K_ICP_ITER, K_ICP_MISC, K_BWD_ZERO, K_TSDF_INTEGRATE, K_TSDF_EXTRACT, K_COUNT
+    K_ICP_BUILD, K_ICP_ITER, K_ICP_MISC, K_BWD_ZERO, K_TSDF_INTEGRATE, K_TSDF_EXTRACT, K_TSDF_RAYCAST, K_COUNT
 };
 
 void prof_begin(int id, cudaStream_t s);

@@ -2,9 +2,10 @@
 `eval_pcd` of SLAM/eval.py:149-223), backed by librtg_splat_b200.so.
 
 * `TsdfVolume`: a dense truncated-signed-distance grid on the device. `integrate` folds one depth frame (a rendered hit
-  depth at a keyframe pose, or a measured depth at a tracked pose) into it; `extract_mesh` runs marching tetrahedra.
-  Both are CUDA kernels of the library (rtg_tsdf_integrate / rtg_tsdf_extract_count / rtg_tsdf_extract_emit); the only
-  host read-back is the two mesh sizes.
+  depth at a keyframe pose, or a measured depth at a tracked pose) into it; `extract_mesh` runs marching tetrahedra;
+  `raycast` renders depth, normal and colour images of that same surface from a pose. All are CUDA kernels of the library
+  (rtg_tsdf_integrate / rtg_tsdf_extract_count / rtg_tsdf_extract_emit / rtg_tsdf_raycast); the only host read-back is
+  the two mesh sizes.
 * `reconstruction_metrics`: accuracy, completion, precision, recall and F-score of a reconstructed point set against
   ground-truth surface points, with eval_pcd's keys and units; nearest neighbours both ways come from `mapsurgery.knn`.
 * `sample_surface`: area-weighted points on a triangle mesh, on the device.
@@ -119,6 +120,33 @@ class TsdfVolume:
         vol = self._desc()
         check(_lib.lib().rtg_tsdf_integrate(C.byref(vol), _p(depth), _p(color), H, W, int(bool(color_channels_last)), fx, fy, cx, cy,
                                             _p(w2c), int(w2c.dtype == torch.float64), _stream(self.device)), "rtg_tsdf_integrate")
+
+    def raycast(self, w2c, intrinsics, H, W):
+        """Renders the surface `extract_mesh` emits from a camera (rtg_tsdf_raycast): {"depth": (H, W) camera z,
+        "normal": (3, H, W) world-space unit normals towards free space, "color": (3, H, W) or None without volume colour},
+        float32 on the volume's device, 0 where the pixel's first crossing is a back face or there is none. w2c: (4, 4)
+        float64 or float32 CUDA tensor, read on the device; intrinsics: (fx, fy, cx, cy). No host synchronisation.
+        As a frame-to-model target for `icp.IcpTracker.update_last_status`: `depth[..., None]` and
+        `normal.permute(1, 2, 0)`, with the frame's normals in world space too."""
+        H, W = int(H), int(W)
+        if H < 1 or W < 1:
+            raise ValueError(f"H and W must be >= 1, got ({H}, {W})")
+        if not isinstance(w2c, torch.Tensor) or not w2c.is_cuda or w2c.dtype not in (torch.float32, torch.float64):
+            raise TypeError("w2c must be a CUDA float32 or float64 tensor")
+        if tuple(w2c.shape) != (4, 4):
+            raise ValueError(f"w2c must be (4, 4), got {tuple(w2c.shape)}")
+        if w2c.device != self.device:
+            raise ValueError("w2c is not on the volume's device")
+        fx, fy, cx, cy = (float(k) for k in intrinsics)
+        w2c = w2c.detach().contiguous()
+        vol = self._desc()
+        dev = self.device
+        depth = torch.empty((H, W), dtype=torch.float32, device=dev)
+        normal = torch.empty((3, H, W), dtype=torch.float32, device=dev)
+        color = torch.empty((3, H, W), dtype=torch.float32, device=dev) if self.color is not None else None
+        check(_lib.lib().rtg_tsdf_raycast(C.byref(vol), _p(w2c), int(w2c.dtype == torch.float64), H, W, fx, fy, cx, cy, _p(depth),
+                                          _p(normal), _p(color), _stream(dev)), "rtg_tsdf_raycast")
+        return {"depth": depth, "normal": normal, "color": color}
 
     def extract_mesh(self):
         """Marching tetrahedra on the Kuhn decomposition of the grid: {"vertices": (V, 3) float32 world positions,
